@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """bench.py -- the headline benchmark of the hot path (BASELINE.json):
 
-    audio-seconds / second (RTFx), tdt-ctc-110m, 10 s clips, 1/2/4/8 x B200
+    audio-seconds / second (RTFx), tdt-ctc-110m, 10 s clips, 1/2/4/8 x H100
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 110m-64x10s|600m-16x30s]
+                    [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 A "step" is one pass of the hot path (PCM -> log-mel -> FastConformer -> TDT greedy) over
@@ -20,6 +21,12 @@ C-ABI (pk_allgather_tokens) inside the timed region: K=16 on 8 GPUs is BASELINE 
            batch i+1 runs under the kernels of batch i); e2e.sync_call = the single blocking call
            pk_transcribe_batch per batch.
   roofline / cpu_baseline / clocks / gpu_launches: see DESIGN.md section "Measurement".
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step returned to its caller, as float64 arrays
+with every entry past a row's length set to 0: the batch configurations the token rows that step appended to the job
+(pk_job_fetch: [length, ids...] per clip) as DIR/tokens.npy; eou-120m-stream the arrays of the last pk_stream_step
+(DIR/len.npy, ids.npy, start.npy, end.npy, conf.npy; one row per stream).  The inputs are seeded, so two builds run with
+the same arguments can be compared output for output.
 
 --impl reference times the reference's own CPU implementation (oracle/_ref/libpkref.so,
 the unmodified reference compiled by oracle/Makefile) on this box's host cores, one 10 s
@@ -66,14 +73,16 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], bf16=d["bf16_tflops"], bf16_sus=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sus=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s.  No sustained figure is measured, so the
+    # data-sheet peak is the denominator too; a card set to a lower power limit cannot reach it.
+    return dict(hbm=3350.0, bf16=989.0, bf16_sus=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, dev):
         super().__init__(daemon=True)
@@ -91,17 +100,17 @@ class ClockSampler(threading.Thread):
     def stop(self):
         if self.proc:
             self.proc.terminate()
-        sm, mx, reasons = [], 0.0, set()
+        sm, mx, reasons, plim = [], 0.0, set(), 0.0
         for r in self.rows:
             try:
-                sm.append(float(r[1])); mx = max(mx, float(r[2]))
+                sm.append(float(r[1])); mx = max(mx, float(r[2])); plim = max(plim, float(r[9]))
                 for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), r[5:9]):
                     if v.lower().startswith("active"):
                         reasons.add(name)
             except Exception:
                 continue
         busy = sorted(sm)[len(sm) // 2:] if sm else [0.0]     # upper half ~ samples under load
-        return {"sm_mhz": float(np.median(busy)), "sm_max_mhz": mx, "reasons": sorted(reasons), "samples": len(sm)}
+        return {"sm_mhz": float(np.median(busy)), "sm_max_mhz": mx, "reasons": sorted(reasons), "samples": len(sm), "power_limit_w": plim}
 
 
 def make_checkpoint(tmpdir, conf=None):
@@ -233,11 +242,14 @@ def run_stream_bench(args, conf):
     streams = [base[i % len(base)] if i < len(base) else np.roll(base[i % len(base)], 4001 * (i // len(base))) for i in range(S)]
     out = eng._tokens(S)
 
+    last = {}
+
     def run(steps, eng_=eng, streams_=streams, out_=out):
         ntok = 0
         for k in range(steps):
             arrs = eng_.stream_step([x[k * CH:(k + 1) * CH] for x in streams_], out=out_, raw=True)
             ntok += int(arrs["len"].sum())
+        last.update(arrs)
         return ntok
 
     run(min(K, 24))                                # warm-up: both chunk patterns seen, graphs instantiated
@@ -253,6 +265,12 @@ def run_stream_bench(args, conf):
     wall = time.perf_counter() - t0
     clocks = sampler.stop()
     launches = eng.launch_count() - l0
+    if args.dump_outputs:           # the arrays the last timed pk_stream_step returned (copied before the latency runs)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        valid = np.arange(eng.cap)[None, :] < last["len"][:, None]
+        np.save(os.path.join(args.dump_outputs, "len.npy"), last["len"].astype(np.float64))
+        for name in ("ids", "start", "end", "conf"):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), np.where(valid, last[name], 0).astype(np.float64))
     audio_s = S * K * CH / 16000.0
     value = audio_s / wall
     # single-stream latency (the reference's case)
@@ -276,13 +294,13 @@ def run_stream_bench(args, conf):
             "data": "synthetic",
             "config": {"workload": f"eou-120m streaming TDT decode, {S} concurrent 16 kHz streams in lock step, {CH}-sample (160 ms) chunks, "
                                    f"{K} chunks per stream ({K * CH / 16000.0:g} s)", "streams": S, "chunk_samples": CH,
-                       "tokens_emitted": ntok, "l2": "weights (435 MB of bf16 hi/lo planes) exceed the 126 MB L2: re-read from HBM every step"},
+                       "tokens_emitted": ntok, "l2": "weights (435 MB of bf16 hi/lo planes) exceed the 50 MB L2: re-read from HBM every step"},
             "e2e": {"value": value, "unit": "x real-time", "h2d_bytes_per_step": S * CH * 4, "d2h_bytes_per_step": int(S * (1 + eng.cap) * 4 + 3 * S * eng.cap * 4),
                     "api": "pk_stream_step per chunk (pageable host PCM in, host token arrays out)"},
             "latency": {"ms_per_chunk_step_all_streams": 1e3 * wall / K, "ms_per_chunk_single_stream": 1e3 * lat1,
                         "real_time_budget_ms": 160.0},
             "gpu_launches": int(launches), "wall_s": wall, "clocks": clocks,
-            "roofline": {"bound": "hbm", "kernel": "the step's tcgen05 GEMMs stream every encoder weight once per step (M = sum of 1-2 frames per stream)",
+            "roofline": {"bound": "hbm", "kernel": "the step's wgmma GEMMs stream every encoder weight once per step (M = sum of 1-2 frames per stream)",
                          "achieved": weight_bytes / (wall / K) / 1e9, "peak": pk["hbm"], "unit": "GB/s",
                          "frac": weight_bytes / (wall / K) / 1e9 / pk["hbm"], "traffic": None,
                          "note": "launch/latency-bound at this S: ~330 kernels per step replayed as one CUDA graph"}}
@@ -316,11 +334,15 @@ def main():
     ap.add_argument("--decoder", default="tdt", choices=["tdt", "ctc"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--tmp", default=os.environ.get("PK_BENCH_TMP", "/tmp/pk_bench"))
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the token rows of the last timed step to DIR/tokens.npy (float64)")
     args = ap.parse_args()
     os.makedirs(args.tmp, exist_ok=True)
     conf = CONFIGS[args.config]
     if args.steps is None:
         args.steps = 375 if conf.get("stream") else 20
+    if args.dump_outputs and args.impl != "ours":
+        raise SystemExit("bench.py: --dump-outputs applies to --impl ours")
     if conf.get("stream"):
         if args.impl == "reference":
             sys.path.insert(0, os.path.join(ROOT, "oracle"))
@@ -431,6 +453,11 @@ def main():
     launches = eng.launch_count() - l0
     rows_all = eng.job_fetch(world * K * BATCH, gathered=True) if world > 1 else eng.job_fetch(K * BATCH)
     mine = rows_all[rank * K * BATCH:(rank + 1) * K * BATCH]
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        rows = mine[(K - 1) * BATCH:K * BATCH].astype(np.float64)
+        rows[np.arange(rows.shape[1])[None, :] > rows[:, :1]] = 0.0       # entries past each row's length are not part of it
+        np.save(os.path.join(args.dump_outputs, "tokens.npy"), rows)
     assert int((rows_all[:, 0] > 0).sum()) == rows_all.shape[0], "bench: an utterance of the job decoded to nothing"
     eng.job_select(0, BATCH)
     eng.run_staged(dec)
@@ -524,26 +551,14 @@ def main():
     gemm_tflops = gemm_fl / max(gemm_ms, 1e-9) / 1e9
     enc_ms = sum(prof[k][0] for k in ("subsample", "gemm", "layernorm", "attention", "dwconv")) / PSTEPS
     math_name = {0: "bf16x3", 1: "bf16", 2: "f32"}[int(cfg.math)]
-    # The timed region is seconds long at ~1 kW: the sustained bf16 peak is the denominator; the burst figure is
-    # reported beside it (frac_of_burst) because short runs keep the boost clock.
-    # DRAM bytes of one launch of the dominant GEMM come from the committed ncu --set full capture
-    # (bench.py cannot run ncu on itself; profiles/*_traffic.json says which launch and how it was taken)
-    traffic, traffic_note = None, None
-    for tf in ("r02_traffic.json", "r01_traffic.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", tf)) as f:
-                tj = json.load(f)
-            traffic, traffic_note = tj["dram_bytes_per_launch"], f'{tj["kernel"]}; {tj["source"]}'
-            break
-        except (OSError, KeyError, ValueError):
-            continue
+    # "peak" is the sustained bf16 rate when MEASURED_PEAKS.json gives one, else the data-sheet figure (see peaks()).
     enc_gflop = conf["enc_gflop"]
-    roofline = {"bound": "tensor", "kernel": "gemm_tc kernels (tcgen05; all GEMM launches of one step)",
+    roofline = {"bound": "tensor", "kernel": "gemm_tc kernels (wgmma; all GEMM launches of one step)",
                 "achieved": gemm_tflops, "peak": pk["bf16_sus"], "unit": "TFLOP/s",
-                "frac": gemm_tflops / pk["bf16_sus"], "frac_of_burst": gemm_tflops / pk["bf16"],
-                "traffic": traffic if args.config == "110m-64x10s" else None, "traffic_of": traffic_note,
+                "frac": gemm_tflops / pk["bf16_sus"], "frac_of_burst": gemm_tflops / pk["bf16"], "power_limit_w": clocks["power_limit_w"],
+                "traffic": None,
                 "mma_frac": (3.0 if int(cfg.math) == 0 else 1.0) * gemm_tflops / pk["bf16_sus"] if int(cfg.math) != 2 else None,
-                "peak_source": pk["src"] + " bf16 sustained (kernel timed inside a long step)",
+                "peak_source": pk["src"] + (" bf16 sustained" if pk["src"] == "measured" else " dense bf16 (not reachable below a 700 W power limit)"),
                 "algorithmic_gflop_per_launch": gemm_fl / max(gemm_n, 1) / 1e9, "launches_per_step": gemm_n // PSTEPS,
                 "avg_launch_ms": gemm_ms / max(gemm_n, 1),
                 "encoder": {"ms_per_clip": enc_ms / BATCH, "ms_per_batch": enc_ms,

@@ -1,4 +1,4 @@
-/* parakeet_b200.h -- the drop-in boundary: a flat C-ABI over the B200-native hot path
+/* parakeet_b200.h -- the drop-in boundary: a flat C-ABI over the H100-native hot path
  *
  *     16 kHz PCM -> log-mel -> FastConformer encoder -> CTC / TDT greedy decode
  *
@@ -39,9 +39,9 @@ typedef enum {
 
 typedef enum { PK_DECODER_CTC = 0, PK_DECODER_TDT = 1 } pk_decoder;
 
-/* GEMM arithmetic.  PK_MATH_BF16X3 (default): tcgen05 kind::f16 MMAs on bf16
+/* GEMM arithmetic.  PK_MATH_BF16X3 (default): wgmma MMAs on bf16
  * hi/lo operand splits, 3 MMAs per product (hi*hi + hi*lo + lo*hi), fp32
- * accumulation in TMEM: ~1e-5 relative, the parity mode.  PK_MATH_BF16X1: hi*hi only
+ * accumulation in registers: ~1e-5 relative, the parity mode.  PK_MATH_BF16X1: hi*hi only
  * (fast, ~4e-3).  PK_MATH_FP32: CUDA-core fp32 GEMM (bring-up / checker). */
 typedef enum { PK_MATH_BF16X3 = 0, PK_MATH_BF16X1 = 1, PK_MATH_FP32 = 2 } pk_math;
 
@@ -239,16 +239,16 @@ pk_status pk_debug_tdt_phases(pk_engine *e, int64_t *out8);
  * {x staging, products, partial store + cluster barrier, DSMEM gather + finalise, number of passes, 0, 0, 0}. */
 pk_status pk_debug_tdt_passes(pk_engine *e, int64_t *out8);
 
-/* GPU self-check of the tcgen05 GEMM kernel against the fp32 CUDA-core GEMM on seeded
+/* GPU self-check of the wgmma GEMM kernel against the fp32 CUDA-core GEMM on seeded
  * random data (epi_kind: EpiKind of csrc/pk_common.cuh; math: PK_MATH_BF16X3 | PK_MATH_BF16X1). */
 pk_status pk_selftest_gemm(int device, int M, int N, int K, int epi_kind, int math, uint32_t seed,
                            float *max_err, float *max_ref);
-/* GPU self-check of the residual GEMM with the LayerNorm fused into its epilogue (csrc/gemm_tc_ln.cu, N = 512, run in place)
+/* GPU self-check of the residual GEMM with the LayerNorm fused into its epilogue (csrc/gemm_tc.cu, N = 512, run in place)
  * against the fp32 GEMM followed by the stand-alone LayerNorm kernel.  mode 0: x = resid + a(A W^T + b), planes = LN1(x);
  * 1: x = LN1(.), planes = LN2(x);  2: x = LN1(.), planes = split(x);  3: mode 0 without a residual.
  * err4 = {max |x - x_ref|, max |x_ref|, max |planes - planes_ref|, max |planes_ref|}. */
 pk_status pk_selftest_gemm_ln(int device, int M, int K, int mode, int math, uint32_t seed, float *err4);
-/* GPU self-check of the tcgen05 attention kernel (csrc/attention_umma.cu: head_dim 64, <= 128 frames per utterance) against the
+/* GPU self-check of the wgmma attention kernel (csrc/attention_wgmma.cu: head_dim 64, <= 128 frames per utterance) against the
  * fp32 CUDA-core attention kernel on seeded random inputs (d_model 512, 8 heads), utterance lengths lens[0..n).  mode bit 0:
  * zero position table; bit 1: zero keys.  err2 = {max |ctx - ctx_ref|, max |ctx_ref|}. */
 pk_status pk_selftest_attention(int device, const int32_t *lens, int n, int tmax, int mode, uint32_t seed, float *err2);

@@ -1,8 +1,8 @@
-"""parakeet.cpp_b200 -- B200-native Parakeet hot path behind the reference's API.
+"""parakeet.cpp_b200 -- H100-native (sm_90a) Parakeet hot path behind the reference's API.
 
     PCM -> log-mel -> FastConformer encoder -> CTC / TDT greedy decode
 
-as hand-written sm_100a CUDA (csrc/) behind the C-ABI of include/parakeet_b200.h.
+as hand-written sm_90a CUDA (csrc/) behind the C-ABI of include/parakeet_b200.h.
 This Python package is only the ctypes binding + harness helpers; the C++
 drop-in shim with the reference's class signatures is include/parakeet/transcribe.hpp.
 

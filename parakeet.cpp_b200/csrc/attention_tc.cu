@@ -3,11 +3,11 @@
 //     S[i,j] = ((q_i + u).k_j + (q_i + v).PP[i-j]) / sqrt(hd),  ctx_i = softmax_j(S[i,:]) V
 // with every product on mma.sync.m16n8k16 (bf16 inputs, fp32 accumulate) using the same hi/lo
 // operand split as the GEMMs (3 MMAs per product: hi.hi + hi.lo + lo.hi), i.e. ~16 mantissa bits,
-// and an fp32 online softmax.  tcgen05 is not used here: per (utterance, head) the matrices are
-// 126 x 126 x 64, far below a UMMA tile pipeline's break-even, and the rel_shift needs a per-row
+// and an fp32 online softmax.  wgmma is not used here: per (utterance, head) the matrices are
+// 126 x 126 x 64, far below a wgmma tile pipeline's break-even, and the rel_shift needs a per-row
 // skew that is natural in registers/shared memory.
 //
-// Operands: the fused q/k/v projection (EPI_QKV_ACT epilogue of the tcgen05 GEMM) writes K | V as bf16 hi/lo
+// Operands: the fused q/k/v projection (EPI_QKV_ACT epilogue of the wgmma GEMM) writes K | V as bf16 hi/lo
 // planes [M, 2d] and q as fp32 [M, d]; PP = pos_emb . Wpos^T is split once at load.  K / V / PP-window tiles
 // are cp.async'ed (16 B) into shared memory and read through ldmatrix (V through .trans).  The CTA forms
 // Qu = q + pos_bias_u and Qv = q + pos_bias_v itself while it builds its Q fragments (one fp32 add and one hi/lo

@@ -1,5 +1,5 @@
 // engine.cu -- the engine behind the C-ABI (include/parakeet_b200.h): weight loading and
-// layout, workspace, and the orchestration of the sm_100a kernels for
+// layout, workspace, and the orchestration of the sm_90a kernels for
 //     PCM -> log-mel -> FastConformer encoder -> CTC / TDT greedy decode.
 //
 // Reference call stack being replaced (SURVEY.md section 3.2/3.3):
@@ -53,7 +53,7 @@ pk_status pk_engine::finish_weight(std::vector<float> &w, std::vector<float> *b,
         out.hi = upload(hi);
         out.lo = upload(lo);
         if (!out.hi || !out.lo) return fail(PK_ERR_CUDA, "cudaMalloc failed (split weight)");
-        if (K % 64 != 0) return fail(PK_ERR_INVALID, "tcgen05 GEMM needs K % 64 == 0");
+        if (K % 64 != 0) return fail(PK_ERR_INVALID, "wgmma GEMM needs K % 64 == 0");
         if (!make_tc_operand(&out.tc, out.hi, out.lo, N, K, tc_tile_n(N)))
             return fail(PK_ERR_CUDA, "cuTensorMapEncodeTiled failed for a weight");
     }
@@ -227,7 +227,6 @@ pk_status pk_engine::load(const char *path) {
                 sp.lo = L.pp_lo;
                 launch_split(L.pp, (size_t)NP * d, sp, stream);
                 ++launches;
-                L.pp_tc_ok = hd == 64 && make_tc_operand(&L.pp_tc, L.pp_hi, L.pp_lo, (uint64_t)NP, (uint64_t)d, 256);
             }
         }
         const std::string cp = lp + "conv_.";
@@ -470,43 +469,20 @@ pk_status pk_engine::upload_shapes() {
 
 // ===================================================================== pipeline
 
-const CUtensorMap *pk_engine::out_map(const void *ptr, bool is_f32, int rows, int ld) {
-    auto key = std::make_tuple(ptr, (int)is_f32, rows, ld);
-    auto it = out_maps.find(key);
-    if (it != out_maps.end()) return &it->second;
-    CUtensorMap m;
-    if (!make_tc_out_map(&m, ptr, is_f32, (uint64_t)rows, (uint64_t)ld)) return nullptr;
-    if (out_maps.size() > 4096) out_maps.clear();          // (shape-varying batches: bounded; maps are rebuilt on demand)
-    return &(out_maps[key] = m);
-}
-
 void pk_engine::gemm(const Act &A, int lda, const GemmWeight &W, int M_, EpiParams epi) {
     epi.bias = W.bias;
-    if (tma_out && cfg.math != PK_MATH_FP32 && epi.kind != EPI_RESID_F32 && M_ > 0) {
-        // results leave the SM through the TMA engine (UTMASTG) wherever the tile is interior (gemm_tc.cu: epilogue_slab64)
-        const bool act_kind = epi.kind == EPI_BIAS_RELU_ACT || epi.kind == EPI_BIAS_SILU_ACT || epi.kind == EPI_BIAS_ACT || epi.kind == EPI_QKV_ACT;
-        if (act_kind && epi.act.hi) {
-            const CUtensorMap *m0 = out_map(epi.act.hi, false, M_, epi.ldo), *m1 = epi.act.lo ? out_map(epi.act.lo, false, M_, epi.ldo) : nullptr;
-            const CUtensorMap *m2 = epi.kind == EPI_QKV_ACT ? out_map(epi.out_f32, true, M_, epi.qcols) : nullptr;
-            if (m0 && (m1 || !epi.act.lo) && (m2 || epi.kind != EPI_QKV_ACT)) { epi.tma_out = 1; epi.tm_out0 = m0; epi.tm_out1 = m1; epi.tm_out2 = m2; }
-        } else if (!act_kind && epi.out_f32) {
-            const CUtensorMap *m0 = out_map(epi.out_f32, true, M_, epi.ldo);
-            if (m0) { epi.tma_out = 1; epi.tm_out0 = m0; }
-        }
-    }
     Scope sc(this, CAT_GEMM, 2.0 * M_ * W.N * W.K);
     if (cfg.math == PK_MATH_FP32) {
         launch_gemm_simt(A.f32, lda, W.w, W.K, M_, W.N, W.K, epi, stream);
     } else if (skinny && M_ <= 128 && skinny_ws && W.N <= 32 * SKINNY_TICKETS) {
         // one row tile: weight-streaming bound -- split over N and K so that every SM pulls weights (gemm_skinny.cu)
-        epi.tma_out = 0;
         cudaError_t ce = launch_gemm_skinny(A.hi, A.lo, lda, W.hi, W.lo, M_, W.N, W.K, cfg.math == PK_MATH_BF16X3, epi, skinny_ws, skinny_ws_floats,
                                             skinny_tickets, SKINNY_TICKETS, num_sms, stream);
         if (ce != cudaSuccess && gemm_err == PK_OK) gemm_err = fail(PK_ERR_CUDA, std::string("skinny GEMM launch: ") + cudaGetErrorString(ce));
     } else {
         const int cl = (gemm_cluster == 2 || gemm_cluster == 4) && lda == W.K ? gemm_cluster : 1;
         cudaError_t ce = launch_gemm_tc(A.tc, W.tc, M_, W.N, W.K, cfg.math == PK_MATH_BF16X3, epi, stream, cl, cl == 4 ? &A.tc32 : &A.tc64);
-        if (ce != cudaSuccess && gemm_err == PK_OK) gemm_err = fail(PK_ERR_CUDA, std::string("tcgen05 GEMM launch: ") + cudaGetErrorString(ce));
+        if (ce != cudaSuccess && gemm_err == PK_OK) gemm_err = fail(PK_ERR_CUDA, std::string("wgmma GEMM launch: ") + cudaGetErrorString(ce));
     }
     ++launches;
 }
@@ -558,8 +534,8 @@ pk_status pk_engine::gemm_ln(const Act &A, int lda, const GemmWeight &W, int M_,
         le.out_ln1 = out_ln1;
         le.planes = planes;
         Scope sc(this, CAT_GEMM, 2.0 * M_ * W.N * W.K);
-        cudaError_t ce = launch_gemm_tc_ln(ln_mcast ? A.tc32 : A.tc, W.tc, M_, W.N, W.K, cfg.math == PK_MATH_BF16X3, le, num_sms, stream);
-        if (ce != cudaSuccess && gemm_err == PK_OK) gemm_err = fail(PK_ERR_CUDA, std::string("tcgen05 GEMM+LayerNorm launch: ") + cudaGetErrorString(ce));
+        cudaError_t ce = launch_gemm_tc_ln(ln_mcast ? A.tc32 : A.tc, W.tc, M_, W.N, W.K, cfg.math == PK_MATH_BF16X3, le, stream);
+        if (ce != cudaSuccess && gemm_err == PK_OK) gemm_err = fail(PK_ERR_CUDA, std::string("wgmma GEMM+LayerNorm launch: ") + cudaGetErrorString(ce));
         ++launches;
         return PK_OK;
     }
@@ -676,17 +652,8 @@ pk_status pk_engine::run_encoder(float *sub_out_host, float *layers_out_host) {
             {
                 Scope sc(this, CAT_ATTENTION);
                 bool ok = false;
-                if (tc_attn && attn_umma && L.pp_tc_ok && relpos_attention_umma_supported(hd, maxT) && ctx.hi) {
-                    // tcgen05 kernel: the k | v planes as a TMA operand of exactly M rows (rows past the batch read as zeros)
-                    auto it = kv_maps.find(M);
-                    if (it == kv_maps.end()) {
-                        if (kv_maps.size() > 256) kv_maps.clear();
-                        TcOperand op;
-                        if (make_tc_operand(&op, qkvp_hi, qkvp_lo, (uint64_t)M, (uint64_t)2 * d, 128)) it = kv_maps.emplace(M, op).first;
-                    }
-                    if (it != kv_maps.end())
-                        ok = launch_relpos_attention_umma(qkv, L.pos_u, L.pos_v, it->second, L.pp_tc, d_row_off, n_utt, maxT, H, hd, Tmax, d, num_sms, ctx, stream);
-                }
+                if (tc_attn && attn_wgmma && relpos_attention_wgmma_supported(hd, maxT))
+                    ok = launch_relpos_attention_wgmma(qkv, L.pos_u, L.pos_v, qkvp_hi, qkvp_lo, 2 * d, d_row_off, n_utt, maxT, H, hd, L.pp_hi, L.pp_lo, Tmax, d, ctx, stream);
                 if (!ok)
                     ok = tc_attn
                         ? launch_relpos_attention_tc(qkv, L.pos_u, L.pos_v, qkvp_hi, qkvp_lo, 2 * d, d_row_off, n_utt, maxT, H, hd, L.pp_hi, L.pp_lo, Tmax, d, ctx, stream)
@@ -923,13 +890,11 @@ pk_status pk_engine_create(const pk_config *cfg, const char *path, int device, p
         g_create_err = "unknown pk_math mode";
         return PK_ERR_INVALID;
     }
-    if (const char *ev = getenv("PK_GEMM_2CTA")) tc_set_2cta(atoi(ev) != 0);
     auto e = std::make_unique<pk_engine>();
     e->cfg = c;
     if (const char *ev = getenv("PK_GRAPH")) e->use_graphs = atoi(ev) != 0;
     if (const char *ev = getenv("PK_ATTN_TC")) e->attn_tc = atoi(ev) != 0;
-    if (const char *ev = getenv("PK_ATTN_UMMA")) e->attn_umma = atoi(ev) != 0;
-    if (const char *ev = getenv("PK_GEMM_TMA_OUT")) e->tma_out = atoi(ev) != 0;
+    if (const char *ev = getenv("PK_ATTN_UMMA")) e->attn_wgmma = atoi(ev) != 0;
     if (const char *ev = getenv("PK_GEMM_SKINNY")) e->skinny = atoi(ev) != 0;
     if (const char *ev = getenv("PK_FUSE_LN")) e->fuse_ln = atoi(ev) != 0;
     if (const char *ev = getenv("PK_GEMM_CLUSTER")) e->gemm_cluster = atoi(ev);
@@ -1040,7 +1005,7 @@ pk_status pk_flush_l2(pk_engine *e) {
     if (!e) return PK_ERR_INVALID;
     cudaSetDevice(e->device);
     if (!e->l2_scratch) {
-        e->l2_scratch_bytes = (size_t)256 << 20;   // > 126 MB L2
+        e->l2_scratch_bytes = (size_t)256 << 20;   // > the 50 MB L2 of an H100
         if (cudaMalloc(&e->l2_scratch, e->l2_scratch_bytes) != cudaSuccess) return e->fail(PK_ERR_CUDA, "cudaMalloc (L2 scratch)");
         e->allocs.push_back(e->l2_scratch);
     }
@@ -1049,13 +1014,11 @@ pk_status pk_flush_l2(pk_engine *e) {
     return PK_OK;
 }
 
-// Runs one GEMM through the tcgen05 kernel and through the fp32 CUDA-core kernel on seeded
+// Runs one GEMM through the wgmma kernel and through the fp32 CUDA-core kernel on seeded
 // random data and returns max |tc - fp32| and max |fp32| (GPU self-check used by the tests).
 pk_status pk_selftest_gemm(int device, int M, int N, int K, int epi_kind, int math, uint32_t seed, float *max_err,
                            float *max_ref) {
     if (cudaSetDevice(device) != cudaSuccess) return PK_ERR_CUDA;
-    if (const char *ev = getenv("PK_GEMM_2CTA")) tc_set_2cta(atoi(ev) != 0);
-    tc_set_debug(getenv("PK_GEMM_DBG") ? atoi(getenv("PK_GEMM_DBG")) : 0);
     if (K % 64 != 0 || (epi_kind == EPI_GLU_F32 && (N & 1))) return PK_ERR_INVALID;
     const int qcols = epi_kind == EPI_QKV_ACT ? N / 3 : 0;     // fused q/k/v projection: N = 3 d -> fp32 q [M, d] + planes [M, 2 d]
     if (epi_kind == EPI_QKV_ACT && (N % 3 != 0 || qcols % 16 != 0)) return PK_ERR_INVALID;
@@ -1104,14 +1067,6 @@ pk_status pk_selftest_gemm(int device, int M, int N, int K, int epi_kind, int ma
         ep.out_f32 = qcols ? q_tc : o_tc;
         ActBuf tc_act; tc_act.hi = oh; tc_act.lo = ol;
         ep.act = tc_act;
-        CUtensorMap om0, om1, om2;
-        if (getenv("PK_GEMM_TMA_OUT") && atoi(getenv("PK_GEMM_TMA_OUT")) && epi_kind != EPI_RESID_F32) {
-            const bool ok = act_out ? (make_tc_out_map(&om0, oh, false, M, No) && make_tc_out_map(&om1, ol, false, M, No))
-                                    : make_tc_out_map(&om0, o_tc, true, M, No);
-            if (ok && (!qcols || make_tc_out_map(&om2, q_tc, true, M, qcols))) {
-                ep.tma_out = 1; ep.tm_out0 = &om0; ep.tm_out1 = act_out ? &om1 : nullptr; ep.tm_out2 = qcols ? &om2 : nullptr;
-            }
-        }
         const bool use_skinny = getenv("PK_SELFTEST_SKINNY") && atoi(getenv("PK_SELFTEST_SKINNY")) && M <= 128;
         float *sws = nullptr;
         unsigned int *stk = nullptr;
@@ -1121,14 +1076,13 @@ pk_status pk_selftest_gemm(int device, int M, int N, int K, int epi_kind, int ma
             cudaMemsetAsync(stk, 0, 1024 * sizeof(unsigned int), st);
             int sms = 0;
             cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-            ep.tma_out = 0;
             for (int rep = 0; rep < 2 && rc == PK_OK; ++rep)      // twice: the tickets must come back to zero
                 if (launch_gemm_skinny(Ah, Al, K, Wh, Wl, M, N, K, math == PK_MATH_BF16X3, ep, sws, (size_t)2 << 20, stk, 1024, sms, st) != cudaSuccess) rc = PK_ERR_CUDA;
             cudaStreamSynchronize(st);
             cudaFree(sws);
             cudaFree(stk);
         } else if (launch_gemm_tc(ta, tw, M, N, K, math == PK_MATH_BF16X3, ep, st, cl, &ta_sl) != cudaSuccess) rc = PK_ERR_CUDA;
-        if (rc == PK_OK && !use_skinny && getenv("PK_SELFTEST_TIME")) {   // warm, back-to-back timing of the tcgen05 launch
+        if (rc == PK_OK && !use_skinny && getenv("PK_SELFTEST_TIME")) {   // warm, back-to-back timing of the wgmma launch
             cudaEvent_t e0, e1;
             cudaEventCreate(&e0); cudaEventCreate(&e1);
             const int reps = 20;
@@ -1139,10 +1093,9 @@ pk_status pk_selftest_gemm(int device, int M, int N, int K, int epi_kind, int ma
             float ms = 0.f;
             cudaEventElapsedTime(&ms, e0, e1);
             const double us = 1e3 * ms / reps, tf = 2.0 * M * N * K / (us * 1e-6) / 1e12;
-            fprintf(stderr, "gemm_tc M=%d N=%d K=%d epi=%d math=%d: %.1f us  %.1f TFLOP/s algorithmic (x%d MMA)  [probe %.0f MHz]\n", M, N, K,
-                    epi_kind, math, us, tf, math == PK_MATH_BF16X3 ? 3 : 1, tc_probe_mhz());
+            fprintf(stderr, "gemm_tc M=%d N=%d K=%d epi=%d math=%d: %.1f us  %.1f TFLOP/s algorithmic (x%d MMA)\n", M, N, K,
+                    epi_kind, math, us, tf, math == PK_MATH_BF16X3 ? 3 : 1);
             cudaEventDestroy(e0); cudaEventDestroy(e1);
-            if (getenv("PK_GEMM_DBG") && (atoi(getenv("PK_GEMM_DBG")) & 32)) tc_print_timeline(8);
         }
     }
     if (cudaStreamSynchronize(st) != cudaSuccess) rc = PK_ERR_CUDA;
@@ -1183,7 +1136,7 @@ pk_status pk_selftest_gemm(int device, int M, int N, int K, int epi_kind, int ma
     return rc;
 }
 
-// GPU self-check of the fused residual-GEMM + LayerNorm kernel (gemm_tc_ln.cu) against the fp32 CUDA-core GEMM followed by
+// GPU self-check of the fused residual-GEMM + LayerNorm kernel (gemm_tc_ln_kernel in gemm_tc.cu) against the fp32 CUDA-core GEMM followed by
 // layernorm_kernel, N = 512.  mode 0: x = resid + a (A W^T + b), planes = LN1(x);  1: x = LN1(.), planes = LN2(x) (block end);
 // 2: x = LN1(.), planes = split(x) (last block);  3: mode 0 without a residual (proj_).  The fused kernel runs IN PLACE
 // (out = resid), as the encoder uses it.  err4 = {max |x - x_ref|, max |x_ref|, max |planes - planes_ref|, max |planes_ref|}.
@@ -1193,8 +1146,6 @@ pk_status pk_selftest_gemm_ln(int device, int M, int K, int mode, int math, uint
     if (K % 64 != 0 || M < 1 || mode < 0 || mode > 3 || !err4) return PK_ERR_INVALID;
     cudaStream_t st;
     cudaStreamCreate(&st);
-    int sms = 0;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     std::vector<float> hA((size_t)M * K), hW((size_t)N * K), hb(N), hr((size_t)M * N), hl(4 * N);
     uint32_t sd = seed * 2654435761u + 777u;
     auto rnd = [&]() { sd = sd * 1664525u + 1013904223u; return ((sd >> 8) & 0xffff) / 32768.0f - 1.0f; };
@@ -1237,12 +1188,11 @@ pk_status pk_selftest_gemm_ln(int device, int M, int K, int mode, int math, uint
     const bool mcast = getenv("PK_LN_MCAST") && atoi(getenv("PK_LN_MCAST")) != 0;
     TcOperand ta128;                              // (the unfused comparison launch needs the 128-row box)
     if (!make_tc_operand(&ta, Ah, Al, M, K, mcast ? 32 : 128) || !make_tc_operand(&ta128, Ah, Al, M, K, 128) || !make_tc_operand(&tw, Wh, Wl, N, K, 128)) rc = PK_ERR_CUDA;
-    gemm_tc_ln_set_debug(getenv("PK_LN_DBG") ? atoi(getenv("PK_LN_DBG")) : 0);
     LnEpi le;
     le.bias = db; le.resid = has_resid ? x_tc : nullptr; le.alpha = ep.alpha; le.out_f32 = x_tc;
     le.ln1_w = w1; le.ln1_b = b1; le.ln2_w = two ? w2 : nullptr; le.ln2_b = two ? b2 : nullptr; le.out_ln1 = out_ln1;
     le.planes.hi = ph; le.planes.lo = math == PK_MATH_BF16X3 ? pl : nullptr;
-    if (rc == PK_OK && launch_gemm_tc_ln(ta, tw, M, N, K, math == PK_MATH_BF16X3, le, sms, st) != cudaSuccess) rc = PK_ERR_CUDA;
+    if (rc == PK_OK && launch_gemm_tc_ln(ta, tw, M, N, K, math == PK_MATH_BF16X3, le, st) != cudaSuccess) rc = PK_ERR_CUDA;
     if (rc == PK_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = PK_ERR_CUDA;
     if (rc == PK_OK) {
         std::vector<float> xr(hr.size()), xt(hr.size()), pr(hr.size());
@@ -1273,7 +1223,7 @@ pk_status pk_selftest_gemm_ln(int device, int M, int K, int mode, int math, uint
         ActBuf tp; tp.hi = ph; tp.lo = pl;
         for (int w = 0; w < 2; ++w) {
             cudaEventRecord(e0, st);
-            for (int i = 0; i < reps; ++i) launch_gemm_tc_ln(ta, tw, M, N, K, math == PK_MATH_BF16X3, le, sms, st);
+            for (int i = 0; i < reps; ++i) launch_gemm_tc_ln(ta, tw, M, N, K, math == PK_MATH_BF16X3, le, st);
             cudaEventRecord(e1, st);
             for (int i = 0; i < reps; ++i) {
                 launch_gemm_tc(ta128, tw, M, N, K, math == PK_MATH_BF16X3, er, st);
@@ -1288,7 +1238,6 @@ pk_status pk_selftest_gemm_ln(int device, int M, int K, int mode, int math, uint
         cudaEventElapsedTime(&ms1, e1, e2);
         fprintf(stderr, "gemm_tc_ln M=%d N=%d K=%d mode=%d math=%d: fused %.1f us | gemm_tc + layernorm %.1f us\n", M, N, K, mode, math,
                 1e3 * ms0 / reps, 1e3 * ms1 / reps);
-        if (getenv("PK_LN_DBG") && atoi(getenv("PK_LN_DBG"))) gemm_tc_ln_print_timeline(2);
         cudaEventDestroy(e0); cudaEventDestroy(e1); cudaEventDestroy(e2);
     }
     for (void *p : {(void *)dA, (void *)dW, (void *)db, (void *)dr, (void *)dl, (void *)x_ref, (void *)x_tc, (void *)p_ref, (void *)Ah, (void *)Al,
@@ -1298,7 +1247,7 @@ pk_status pk_selftest_gemm_ln(int device, int M, int K, int mode, int math, uint
     return rc;
 }
 
-// GPU self-check of the tcgen05 attention kernel (attention_umma.cu) against the fp32 CUDA-core attention kernel on seeded
+// GPU self-check of the wgmma attention kernel (attention_wgmma.cu) against the fp32 CUDA-core attention kernel on seeded
 // random q | k | v, position table and biases: d_model 512, 8 heads of 64, utterance lengths lens[0..n) (<= 128), table for
 // `tmax` frames.  mode bit 0: zero position table (isolates Qu.K^T -> softmax -> P.V); bit 1: zero keys (isolates the
 // rel_shift path).  err2 = {max |ctx - ctx_ref|, max |ctx_ref|}.
@@ -1355,13 +1304,28 @@ pk_status pk_selftest_attention(int device, const int32_t *lens, int n, int tmax
     ActBuf ref; ref.f32 = c_ref;
     pk_status rc = PK_OK;
     if (!launch_relpos_attention(dq, 3 * d, doff, n, maxT, H, hd, dpp, tmax, du, dv, d, ref, st)) rc = PK_ERR_INVALID;
-    TcOperand kv, pp;
-    if (rc == PK_OK && (!make_tc_operand(&kv, kvh, kvl, (uint64_t)M, (uint64_t)2 * d, 128) || !make_tc_operand(&pp, pph, ppl, (uint64_t)NP, (uint64_t)d, 256))) rc = PK_ERR_CUDA;
     ActBuf got; got.hi = ch; got.lo = cl;
-    int sms = 0;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    relpos_attention_umma_set_debug(getenv("PK_AU_DBG") ? atoi(getenv("PK_AU_DBG")) : 0);
-    if (rc == PK_OK && !launch_relpos_attention_umma(dq32, du, dv, kv, pp, doff, n, maxT, H, hd, tmax, d, sms, got, st)) rc = PK_ERR_INVALID;
+    if (rc == PK_OK && !launch_relpos_attention_wgmma(dq32, du, dv, kvh, kvl, 2 * d, doff, n, maxT, H, hd, pph, ppl, tmax, d, got, st)) rc = PK_ERR_INVALID;
+    if (rc == PK_OK && getenv("PK_SELFTEST_TIME")) {    // warm back-to-back: the wgmma kernel vs the mma.sync kernel
+        cudaEvent_t e0, e1, e2;
+        cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventCreate(&e2);
+        const int reps = 50;
+        for (int w = 0; w < 2; ++w) {
+            cudaEventRecord(e0, st);
+            for (int i = 0; i < reps; ++i) launch_relpos_attention_wgmma(dq32, du, dv, kvh, kvl, 2 * d, doff, n, maxT, H, hd, pph, ppl, tmax, d, got, st);
+            cudaEventRecord(e1, st);
+            for (int i = 0; i < reps; ++i) launch_relpos_attention_tc(dq32, du, dv, kvh, kvl, 2 * d, doff, n, maxT, H, hd, pph, ppl, tmax, d, got, st);
+            cudaEventRecord(e2, st);
+            cudaStreamSynchronize(st);
+        }
+        float ms0 = 0.f, ms1 = 0.f;
+        cudaEventElapsedTime(&ms0, e0, e1);
+        cudaEventElapsedTime(&ms1, e1, e2);
+        fprintf(stderr, "attention n_utt=%d maxT=%d: wgmma %.1f us | mma.sync %.1f us per launch\n", n, maxT, 1e3 * ms0 / reps, 1e3 * ms1 / reps);
+        cudaEventDestroy(e0); cudaEventDestroy(e1); cudaEventDestroy(e2);
+        // the timing launches overwrote ctx with the mma.sync result: run the checked kernel again
+        launch_relpos_attention_wgmma(dq32, du, dv, kvh, kvl, 2 * d, doff, n, maxT, H, hd, pph, ppl, tmax, d, got, st);
+    }
     if (rc == PK_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = PK_ERR_CUDA;
     if (rc == PK_OK) {
         std::vector<float> r((size_t)M * d);
@@ -1376,25 +1340,6 @@ pk_status pk_selftest_attention(int device, const int32_t *lens, int n, int tmax
             mr = std::max(mr, std::fabs(r[i]));
         }
         err2[0] = me; err2[1] = mr;
-    }
-    if (rc == PK_OK && getenv("PK_SELFTEST_TIME")) {
-        cudaEvent_t e0, e1, e2;
-        cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventCreate(&e2);
-        const int reps = 20;
-        for (int w = 0; w < 2; ++w) {
-            cudaEventRecord(e0, st);
-            for (int i = 0; i < reps; ++i) launch_relpos_attention_umma(dq32, du, dv, kv, pp, doff, n, maxT, H, hd, tmax, d, sms, got, st);
-            cudaEventRecord(e1, st);
-            for (int i = 0; i < reps; ++i) launch_relpos_attention_tc(dq32, du, dv, kvh, kvl, 2 * d, doff, n, maxT, H, hd, pph, ppl, tmax, d, got, st);
-            cudaEventRecord(e2, st);
-            cudaStreamSynchronize(st);
-        }
-        float ms0 = 0.f, ms1 = 0.f;
-        cudaEventElapsedTime(&ms0, e0, e1);
-        cudaEventElapsedTime(&ms1, e1, e2);
-        fprintf(stderr, "attention n_utt=%d maxT=%d: tcgen05 %.1f us | mma.sync %.1f us\n", n, maxT, 1e3 * ms0 / reps, 1e3 * ms1 / reps);
-        if (getenv("PK_AU_DBG") && atoi(getenv("PK_AU_DBG"))) relpos_attention_umma_print_timeline(n < 32 ? 1 : 4);
-        cudaEventDestroy(e0); cudaEventDestroy(e1); cudaEventDestroy(e2);
     }
     for (void *p : {(void *)dq, (void *)dq32, (void *)dkv, (void *)dpp, (void *)du, (void *)dv, (void *)c_ref, (void *)kvh, (void *)kvl, (void *)pph,
                     (void *)ppl, (void *)ch, (void *)cl, (void *)doff})

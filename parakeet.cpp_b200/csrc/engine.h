@@ -35,17 +35,17 @@ std::string &create_err();   // last error of a failed pk_engine_create / engine
 
 inline int conv_len(int L) { return (L - 1) / 2 + 1; }  // k3 s2 p1 (operations.cpp:3191-3196)
 
-// A linear layer's parameters on the device: fp32 master [N][K] + bias, and (tcgen05
+// A linear layer's parameters on the device: fp32 master [N][K] + bias, and (wgmma
 // modes) the bf16 hi/lo split planes of the weight.
 struct GemmWeight {
     float *w = nullptr;
     bf16 *hi = nullptr, *lo = nullptr;
     float *bias = nullptr;
     int N = 0, K = 0;
-    TcOperand tc;   // TMA tensor maps of hi/lo (tcgen05 modes)
+    TcOperand tc;   // TMA tensor maps of hi/lo (wgmma modes)
 };
 
-// An activation buffer that feeds GEMMs, with its TMA tensor maps (tcgen05 modes).
+// An activation buffer that feeds GEMMs, with its TMA tensor maps (wgmma modes).
 struct Act : ActBuf {
     TcOperand tc;
     TcOperand tc32, tc64;   // the same planes with a 32- / 64-row box (A tiles fetched in slices and TMA-multicast across a 4- / 2-CTA cluster)
@@ -59,8 +59,6 @@ struct LayerW {
     float *pos_u, *pos_v;
     float *pp;  // [(2*Tmax-1)][d] projected relative-position table
     bf16 *pp_hi = nullptr, *pp_lo = nullptr;   // its bf16 split planes (tensor-core attention)
-    TcOperand pp_tc;                           // their TMA maps, box 64 x 256 (tcgen05 attention: one box = every relative position of a 128 x 128 tile)
-    bool pp_tc_ok = false;
     float *conv_ln_w, *conv_ln_b;
     GemmWeight pw1, pw2;
     float *dw_w, *dw_b;  // BatchNorm folded; [d][k]
@@ -141,8 +139,9 @@ struct pk_engine {
     struct GraphEntry { cudaGraphExec_t exec = nullptr; int64_t launches = 0; int seen = 0; };
     std::map<std::string, GraphEntry> graphs;
     bool use_graphs = true;
-    bool attn_umma = true;                     // tcgen05 attention (attention_umma.cu) for head_dim 64 and batches of <= 128-frame utterances (PK_ATTN_UMMA=0: mma.sync kernel)
-    std::map<int, TcOperand> kv_maps;          // TMA maps of the k | v planes, keyed by the number of rows of the batch
+    bool attn_wgmma = false;                   // PK_ATTN_UMMA=1 (the switch's name from the earlier design): wgmma attention (attention_wgmma.cu)
+                                               // for head_dim 64 and batches of <= 128-frame utterances.  Off by default: measured on H100 (700 W),
+                                               // 64 x 126 frames, 89 us per launch against 69 us for the mma.sync kernel
     bool attn_tc = true;                       // mma.sync attention for head_dim 64 / 128 (PK_ATTN_TC=0: fp32 kernel)
 
     // ---- the staged batch
@@ -245,19 +244,15 @@ struct pk_engine {
     pk_status set_batch_shapes(const int32_t *n_frames_or_null, const int64_t *offsets_or_null, int n);
     pk_status upload_shapes();
     void gemm(const Act &A, int lda, const GemmWeight &W, int M_, EpiParams epi);
-    // x = resid + alpha * (A . W^T + b) followed by LayerNorm(s): ONE kernel (gemm_tc_ln.cu) when fuse_ln applies,
+    // x = resid + alpha * (A . W^T + b) followed by LayerNorm(s): ONE kernel (gemm_tc_ln_kernel) when fuse_ln applies,
     // else the residual GEMM and layernorm_kernel.  resid_in_x: the residual is x itself (false: x = A . W^T + b).
     // out_ln1: x receives LayerNorm_1 of the sum (block end) instead of the sum; planes = split of the last LayerNorm.
     pk_status gemm_ln(const Act &A, int lda, const GemmWeight &W, int M_, bool resid_in_x, float alpha, const float *ln1_w, const float *ln1_b,
                       bool out_ln1, const float *ln2_w, const float *ln2_b, ActBuf planes);
     int gemm_cluster = 0;                      // PK_GEMM_CLUSTER=2|4: wide GEMMs (fc1, q/k/v, pw1) run as clusters of 2 | 4 CTAs along N with the A tile multicast
-    bool ln_mcast = false;                     // PK_LN_MCAST=1: the A tile is fetched in quarters and TMA-multicast across the cluster (measured: no gain)
-    int fuse_ln_min_k = 0;                     // PK_FUSE_LN_MINK: fuse only GEMMs with K >= this (short-K launches are epilogue-bound either way)
+    bool ln_mcast = false;                     // PK_LN_MCAST=1: the A tile is fetched in quarters and TMA-multicast across the cluster
+    int fuse_ln_min_k = 0;                     // PK_FUSE_LN_MINK: fuse only GEMMs with K >= this
     bool fuse_ln = false;                      // PK_FUSE_LN=1: LayerNorm in the epilogue of the GEMM that produces its input
-    // output-side tensor maps of the TMA-store epilogue, keyed by (buffer, leading dimension, rows)
-    std::map<std::tuple<const void *, int, int, int>, CUtensorMap> out_maps;
-    const CUtensorMap *out_map(const void *ptr, bool is_f32, int rows, int ld);
-    bool tma_out = true;                       // PK_GEMM_TMA_OUT=0: results leave through st.global instead
     // few-row GEMMs (M <= 128: streaming steps, short utterances) go to gemm_skinny.cu (PK_GEMM_SKINNY=0: never)
     bool skinny = true;
     float *skinny_ws = nullptr;

@@ -1,7 +1,7 @@
 // gemm_simt.cu -- fp32 CUDA-core GEMM  C = epi(A[M,K] . W[N,K]^T + bias)
 //
 // This is the PK_MATH_FP32 arithmetic: exact fp32 products and fp32 accumulation,
-// used for bring-up, as the on-device checker of the tcgen05 kernel (gemm_tc.cu), and
+// used for bring-up, as the on-device checker of the wgmma kernel (gemm_tc.cu), and
 // for the small load-time GEMMs (pos_proj of the position table, the LSTM input table).
 // It computes what nn::Linear (axiom linear.cpp:15-27) and the k=1 / 1x1 convolutions
 // (operations.cpp:2960, :3133) compute, with the activation/residual that follows

@@ -1,8 +1,8 @@
 // gemm_skinny.cu -- the GEMM for FEW ROWS (M <= 128): C = epi(A[M,K] . W[N,K]^T + bias) with the same bf16 hi/lo operand
-// planes and the same 3-MMA split (hi.hi + hi.lo + lo.hi, fp32 accumulate) as the tcgen05 kernel (gemm_tc.cu), for the
+// planes and the same 3-MMA split (hi.hi + hi.lo + lo.hi, fp32 accumulate) as the wgmma kernel (gemm_tc.cu), for the
 // launches where that kernel cannot fill the machine: the streaming path (SURVEY.md section 8f row 2) advances S streams by
 // 1-2 encoder frames per step, so every encoder GEMM has M = S .. 2S rows -- ONE 128-row tile -- and the persistent
-// tcgen05 grid shrinks to N/128 CTAs (4 for the N = 512 layers) that walk K serially (32 k-blocks for fc2).  Such a
+// wgmma grid shrinks to N/128 CTAs (4 for the N = 512 layers) that walk K serially (32 k-blocks for fc2).  Such a
 // GEMM is weight-streaming bound: 4 bytes per weight, each read once.
 //
 // Decomposition: CTA = (32 output columns, one slice of K); the grid is sized to ~2 CTAs per SM by splitting K, so all

@@ -1,34 +1,27 @@
-// gemm_tc.cu -- K5: the tensor-core GEMM of the encoder, hand-written for sm_100a:
+// gemm_tc.cu -- K5: the tensor-core GEMM of the encoder, hand-written for sm_90a:
 //     C = epi(A[M,K] . W[N,K]^T + bias)
-// TMA (cp.async.bulk.tensor, SWIZZLE_128B) -> shared memory -> tcgen05.mma (UMMA, one
-// issuing thread, cta_group::1, M=128 x N=BN x K=16 per instruction) -> fp32 accumulator in
-// TMEM -> tcgen05.ld -> fused epilogue (pk_common.cuh: bias / ReLU / SiLU / GLU / residual,
-// output either fp32 or the bf16 hi/lo operand planes of the next GEMM).
+// TMA (cp.async.bulk.tensor, SWIZZLE_128B) -> shared-memory stages -> wgmma (m64 x BN x k16, bf16 operands straight
+// from shared memory, fp32 accumulator in registers) -> fused epilogue from registers (pk_common.cuh: bias / ReLU /
+// SiLU / GLU / residual, output either fp32 or the bf16 hi/lo operand planes of the next GEMM).
 //
 // Arithmetic (pk_math): operands are bf16 hi/lo SPLITS of the fp32 values
 // (hi = rn_bf16(x), lo = rn_bf16(x - hi); weights split once at load, activations split by
 // the producing kernel's epilogue).  PK_MATH_BF16X3 issues three MMAs per product,
-//     A_hi.W_hi + A_hi.W_lo + A_lo.W_hi      (fp32 accumulate in TMEM)
-// which keeps ~16 mantissa bits (measured: encoder output 8e-6 rel vs 4e-3 for plain bf16
-// and 6e-4 for TF32) -- the reference is an fp32 CPU build and parity is token-identical.
+//     A_hi.W_hi + A_hi.W_lo + A_lo.W_hi      (fp32 accumulate)
+// which keeps ~16 mantissa bits -- the reference is an fp32 CPU build and parity is token-identical.
 // PK_MATH_BF16X1 issues only A_hi.W_hi.
 //
-// Structure (persistent, one CTA per SM, 320 threads, static round-robin tile schedule):
-//   warp 0      TMA producer   : waits empty[s], arms full[s] with the byte count, issues
-//                                the 2 or 4 tile loads of k-block kb into stage s
-//   warp 1      MMA issuer     : allocates TMEM (2 x BN columns: the accumulator is double
-//                                buffered); per tile waits acc_empty[b]; per k-block waits
-//                                full[s], 4 x (1|3) tcgen05.mma, tcgen05.commit -> empty[s];
-//                                after the last k-block tcgen05.commit -> acc_full[b]
-//   warps 2..9  epilogue       : wait acc_full[b]; tcgen05.ld 32 lanes x 16 columns (warp w owns
-//                                TMEM lanes 32*(w%4).., half (w-2)/4 of the columns); release
-//                                acc_empty[b] after the last read; transpose through shared
-//                                memory so global stores are row-contiguous; epilogue4 per 4 cols
-// so the epilogue of tile i overlaps the MMAs of tile i+1.
+// Structure (persistent, one CTA per SM, 384 threads = three warpgroups, static round-robin tile schedule, n-tile
+// fastest so that concurrently running CTAs share the same A rows through L2):
+//   warpgroup 0     TMA producer : one elected thread waits empty[s], arms full[s] with the byte count and issues the
+//                                  2 or 4 tile loads of k-block kb into stage s; it runs ahead across tiles, so the
+//                                  loads of tile i+1 overlap the epilogue of tile i
+//   warpgroups 1-2  consumers    : rows [64 (wg - 1), 64 wg) of the 128-row tile; per k-block wait full[s], 4 x (1|3)
+//                                  wgmma, commit; one wgmma group stays in flight and the stage of the previous
+//                                  k-block is released (empty[s], one arrival per consumer warp) once it has retired;
+//                                  then the epilogue straight from the accumulator registers
 // Every spin-wait is bounded and traps, so a protocol bug is an error, not a hung GPU.
 #include <cuda.h>
-
-#include <cstdio>
 
 #include "kernels.h"
 #include "tc_prims.cuh"
@@ -38,718 +31,285 @@ namespace {
 
 using namespace tc;
 
-__device__ int g_l2_hint_mode;   // measurement aid (PK_GEMM_DBG bits 10-11): 0 = loads EVICT_LAST, 1 = no hints, 2 = + stores EVICT_FIRST
+constexpr int TC_THREADS = 384;
+constexpr int CONSUMER_WARPS = 8;
 
-constexpr int STG_LD = 20;                      // epilogue staging row stride (floats): 16 columns + pad
-
-// Global operands of one 16-column chunk (this lane: 4 rows x 4 columns), issued one chunk AHEAD of
-// their use so that the L2 round trip overlaps the previous chunk's transpose / math / stores.
-struct EpiOperands {
-    float4 b, r[4];
-};
-template <int EK>
-__device__ __forceinline__ void epi_load(const EpiParams &epi, int rb, int gc, int M, bool ok, EpiOperands &o) {
-    o.b = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (EK == EPI_RESID_F32) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) o.r[i] = o.b;
-    }
-    if (ok) {
-        if (epi.bias) o.b = __ldg(reinterpret_cast<const float4 *>(epi.bias + gc));
-        if (EK == EPI_RESID_F32) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-                if (rb + i * 8 < M) o.r[i] = *reinterpret_cast<const float4 *>(epi.resid + (size_t)(rb + i * 8) * epi.ldo + gc);
-        }
-    }
-}
-
-// Epilogue of one warp's slab of an accumulator tile: TMEM lanes [32q, 32q+32) x NCOLS fp32 columns
-// starting at `taddr`; output rows row0.., global columns gcol0...  The slab is processed in 16-column
-// chunks; chunk c+1's TMEM read and global operands (bias / residual) are issued before chunk c is
-// transposed through this warp's staging buffer (lane = TMEM row -> 8 rows x 4 lanes x float4, so
-// global stores are 64 B-contiguous per row), which hides both latencies.  The loop is deliberately
-// NOT unrolled: the body is ~150 instructions and the kernels must stay inside the instruction
-// cache.  `release()` is called once, as soon as the last TMEM read has landed, so the MMA warp can
-// start refilling this accumulator buffer while the tail is still being stored.
-template <int NCOLS, int EK, typename ReleaseFn>
-__device__ __forceinline__ void epilogue_slab(uint32_t taddr, uint32_t stg_s, int row0, int gcol0, int M, int N,
-                                              const EpiParams &epi_param, int lane, ReleaseFn release, int dbg = 0) {
-    // Register copy of the parameters for the fast path.  (The out-of-line edge path takes the
-    // struct by reference; reading fields through that same object here makes every pointer a
-    // generic-address reload after each store.)
-    const EpiParams epi = epi_param;
-    constexpr int NCH = NCOLS / 16;
-    static_assert(NCOLS % 16 == 0 && NCH >= 1, "slab width");
-    const int cc = (lane & 3) * 4, rb = row0 + (lane >> 2);
-    const bool vec_ok = ((epi.ldo & 3) == 0) && ((N & 3) == 0);
-    uint32_t vc[16], vn[16];
-    EpiOperands oc, on;
-    tmem_ld16_issue(taddr, vc);
-    epi_load<EK>(epi, rb, gcol0 + cc, M, vec_ok && gcol0 + 16 <= N, oc);
-    tmem_wait_ld();
-    if (NCH == 1) release();
-#pragma unroll 1
-    for (int ch = 0; ch < NCH; ++ch) {
-        const int gc0 = gcol0 + ch * 16;
-        const bool interior = vec_ok && (gc0 + 16 <= N);
-        const bool has_next = ch + 1 < NCH;
-        if (has_next) {
-            tmem_ld16_issue(taddr + (uint32_t)(ch + 1) * 16u, vn);
-            epi_load<EK>(epi, rb, gc0 + 16 + cc, M, vec_ok && gc0 + 32 <= N, on);
-        }
-        if (!(dbg & 4)) {       // (measurement aid, bit 2: TMEM drain only)
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-            sts128(stg_s + (uint32_t)(lane * STG_LD + 4 * j) * 4u, vc[4 * j], vc[4 * j + 1], vc[4 * j + 2], vc[4 * j + 3]);
-        __syncwarp();
-        float4 val[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) val[i] = lds128(stg_s + (uint32_t)((i * 8 + (lane >> 2)) * STG_LD + cc) * 4u);
-        if (interior) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) val[i] = epi_math<EK>(val[i], oc.b, oc.r[i], epi.alpha);
-            if (dbg & 8) {      // (measurement aid, bit 3: everything but the global stores)
-                if (val[0].x + val[1].y + val[2].z + val[3].w == 1.2345e-30f) epi_store<EK>(epi, rb, gc0 + cc, val[0]);
-            } else {
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-                if (rb + i * 8 < M) epi_store<EK>(epi, rb + i * 8, gc0 + cc, val[i]);
-            }
-        } else {
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-                if (rb + i * 8 < M) epilogue4(epi_param, rb + i * 8, gc0 + cc, N, val[i]);
-        }
-        }
-        __syncwarp();
-        if (has_next) {
-            tmem_wait_ld();
-            if (ch + 2 == NCH) release();
-#pragma unroll
-            for (int j = 0; j < 16; ++j) vc[j] = vn[j];
-            oc.b = on.b;
-            if (EK == EPI_RESID_F32) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) oc.r[i] = on.r[i];
-            }
-        }
-    }
-}
-
-// measurement aid: SM cycles and nanoseconds CTA 0 spent in its epilogue loop (effective SM clock under this kernel)
-__device__ unsigned long long g_clk_probe[2];
-// measurement aid (debug bit 5): per-tile timeline of CTA 0 -- [tile][0..3] = MMA thread: accumulator free, last MMA issued;
-// epilogue warp 2: accumulator full seen, tile stored.  (clock64 of SM 0's CTA)
-__device__ long long g_timeline[64][8];   // [4..6]: epilogue sub-phases of warp 2 (TMEM loads landed, maths done, first plane handed to the store path)
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Wide epilogue (interior tiles): one warp drains a 32-row x 64-column slab of the accumulator.
-// Measured on B200 (profiles/r02_gemm_timeline.txt): the 16-column epilogue above spent ~9000 cycles per 128 x 128
-// tile against ~7300 for the tile's MMAs -- 40 % of it in global stores that wrote 32-byte pieces of 8 different rows
-// per instruction (one L2 request per 32 B sector).  Here every global store (and residual load) instruction covers
-// four FULL 128-byte lines: a lane first finishes its own row in registers (tcgen05.ld 32x32b.x32 x 2 -> 64 columns,
-// bias / activation / bf16 split applied row-wise, bias fetched by warp-uniform broadcast loads), writes 128 B of it
-// into the warp's 4 KB staging tile (16-byte pieces XOR-swizzled by the row: conflict-free both ways), and the warp
-// reads the tile back transposed -- lane = (row it*4 + lane/8, piece lane%8) -- so 8 lanes cover one 128-byte line.
-// The accumulator buffer is released as soon as the two TMEM loads have landed, long before the stores.
-constexpr int STGW_BYTES = 4096;                // per-warp staging tile of the wide epilogue: 32 rows x 128 B
-
-// lane's 128-byte row segment (32 words) -> staging; then the warp stores the 32 x 128 B tile to global memory, rows
-// row0 .. row0+31 at `base + row * ld_bytes` (base already includes the column offset).  RESID: out = resid + value.
-__device__ int g_store_mode;    // measurement aid: 0 = st.global, 1 = st.global.cs (evict-first), 2 = st.global.wt
-__device__ __forceinline__ void stg128(void *p, const uint4 &v, int mode) {
-    if (mode == 1)
-        asm volatile("st.global.cs.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-    else if (mode == 2)
-        asm volatile("st.global.wt.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-    else
-        *reinterpret_cast<uint4 *>(p) = v;
-}
-template <bool RESID>
-__device__ __forceinline__ void store_tile128(uint32_t stg_s, int lane, const uint32_t *r, uint8_t *base, const uint8_t *rbase,
-                                              size_t ld_bytes, int row0, int M) {
-    const int smode = g_store_mode;
-    uint4 rr[8];
-    if (RESID) {        // residual pieces in the transposed (coalesced) pattern, in flight while the tile is staged
-#pragma unroll
-        for (int it = 0; it < 8; ++it) {
-            const int row = it * 4 + (lane >> 3);
-            rr[it] = make_uint4(0u, 0u, 0u, 0u);
-            if (row0 + row < M) rr[it] = *reinterpret_cast<const uint4 *>(rbase + (size_t)(row0 + row) * ld_bytes + ((lane & 7) << 4));
-        }
-    }
-#pragma unroll
-    for (int c = 0; c < 8; ++c)
-        sts128(stg_s + (uint32_t)(lane * 128 + ((c ^ (lane & 7)) << 4)), r[4 * c], r[4 * c + 1], r[4 * c + 2], r[4 * c + 3]);
-    __syncwarp();
-#pragma unroll
-    for (int it = 0; it < 8; ++it) {
-        const int row = it * 4 + (lane >> 3), c = lane & 7;
-        uint4 v = lds128u(stg_s + (uint32_t)(row * 128 + ((c ^ (row & 7)) << 4)));
-        if (RESID) {
-            v.x = __float_as_uint(__uint_as_float(rr[it].x) + __uint_as_float(v.x));
-            v.y = __float_as_uint(__uint_as_float(rr[it].y) + __uint_as_float(v.y));
-            v.z = __float_as_uint(__uint_as_float(rr[it].z) + __uint_as_float(v.z));
-            v.w = __float_as_uint(__uint_as_float(rr[it].w) + __uint_as_float(v.w));
-        }
-        if (row0 + row < M) stg128(base + (size_t)(row0 + row) * ld_bytes + (c << 4), v, smode);
-    }
-    __syncwarp();
-}
-
-// The same 32 x 128 B tile leaves through the TMA engine: staged exactly in the SWIZZLE_128B layout of the output map
-// (16-byte chunk c of row r at chunk c ^ (r & 7): what store_tile128 writes), one lane issues cp.async.bulk.tensor
-// shared -> global (rows past M are clipped by the map) and waits until the engine has read the tile.
-__device__ __forceinline__ void stg_acquire(int lane) {    // the TMA engine has finished READING this warp's staging tile
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    __syncwarp();
-}
-__device__ __forceinline__ void tma_store_tile(uint32_t stg_s, int lane, const uint32_t *r, const CUtensorMap *tm, int col, int row0) {
-    stg_acquire(lane);          // waits for the PREVIOUS store of this warp only now: its read overlapped the maths in between
-#pragma unroll
-    for (int c = 0; c < 8; ++c)
-        sts128(stg_s + (uint32_t)(lane * 128 + ((c ^ (lane & 7)) << 4)), r[4 * c], r[4 * c + 1], r[4 * c + 2], r[4 * c + 3]);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy writes -> visible to the async proxy
-    __syncwarp();
-    if (lane == 0) {
-        if (g_l2_hint_mode == 2)
-            asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], %4;"
-                         ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(stg_s), "r"(col), "r"(row0), "l"(L2_EVICT_FIRST) : "memory");
-        else
-        asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                     ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(stg_s), "r"(col), "r"(row0) : "memory");
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-    }
-}
-
-
-// Can the slab [gcol0, gcol0 + 64) of this launch take the wide path?  (warp-uniform)
-template <int EK>
-__device__ __forceinline__ bool wide_ok(const EpiParams &epi, int gcol0, int N) {
-    if (gcol0 + 64 > N) return false;
-    if (EK == EPI_BIAS_F32 || EK == EPI_BIAS_RELU_F32 || EK == EPI_RESID_F32) return (epi.ldo & 3) == 0;
-    if (EK == EPI_GLU_F32) return (epi.ldo & 3) == 0;
-    if (EK == EPI_QKV_ACT) return (epi.ldo & 7) == 0 && (epi.qcols & 63) == 0 && epi.act.hi != nullptr && epi.out_f32 != nullptr;
-    return (epi.ldo & 7) == 0 && epi.act.hi != nullptr;
-}
-
-template <int EK, typename ReleaseFn>
-__device__ __forceinline__ void epilogue_slab64(uint32_t taddr, uint32_t stg_s, int row0, int gcol0, int M, const EpiParams &epi_param,
-                                                int lane, ReleaseFn release, bool last_slab, const CUtensorMap *tm0, const CUtensorMap *tm1,
-                                                const CUtensorMap *tm2, long long *tl = nullptr) {
-    const EpiParams epi = epi_param;
-    const bool tma = epi.tma_out != 0;
-    uint32_t a0[32], a1[32];
-    tmem_ld32_issue(taddr, a0);
-    tmem_ld32_issue(taddr + 32u, a1);
-    tmem_wait_ld();
-    if (last_slab) release();
-    if (tl) tl[4] = clock64();
-    // row-wise on 32 columns [c0, c0 + 32) of the slab: + bias (warp-uniform float4 loads), activation
-    auto rowmath = [&](const uint32_t (&a)[32], int c0, float (&v)[32]) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-            float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (epi.bias) b = __ldg(reinterpret_cast<const float4 *>(epi.bias + gcol0 + c0 + j));
-            v[j] = __uint_as_float(a[j]) + b.x;
-            v[j + 1] = __uint_as_float(a[j + 1]) + b.y;
-            v[j + 2] = __uint_as_float(a[j + 2]) + b.z;
-            v[j + 3] = __uint_as_float(a[j + 3]) + b.w;
-        }
-        if (EK == EPI_BIAS_RELU_F32 || EK == EPI_BIAS_RELU_ACT) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-        } else if (EK == EPI_BIAS_SILU_ACT) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] *= fast_sigmoid(v[j]);
-        } else if (EK == EPI_RESID_F32) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] *= epi.alpha;
-        }
-    };
-    const bool q_part = (EK == EPI_QKV_ACT) && gcol0 < epi.qcols;      // warp-uniform; compile-time false for the other kinds
-    if (EK == EPI_BIAS_F32 || EK == EPI_BIAS_RELU_F32 || EK == EPI_RESID_F32 || q_part) {
-        // fp32 rows: 256 B per lane -> two 128-byte passes  (EPI_QKV_ACT: the q columns, matrix [M, qcols])
-        const int ldf = (EK == EPI_QKV_ACT) ? epi.qcols : epi.ldo;
-        const CUtensorMap *tmf = (EK == EPI_QKV_ACT) ? tm2 : tm0;
-        uint8_t *ob = reinterpret_cast<uint8_t *>(epi.out_f32 + gcol0);
-        const uint8_t *rb = reinterpret_cast<const uint8_t *>(epi.resid + gcol0);
-        const size_t ldb = (size_t)ldf * 4;
-        {
-            float v[32];
-            rowmath(a0, 0, v);
-            uint32_t r[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(v[j]);
-            if (tl) tl[5] = clock64();
-            if (tma && EK != EPI_RESID_F32) tma_store_tile(stg_s, lane, r, tmf, gcol0, row0);
-            else store_tile128<EK == EPI_RESID_F32>(stg_s, lane, r, ob, rb, ldb, row0, M);
-            if (tl) tl[6] = clock64();
-        }
-        {
-            float v[32];
-            rowmath(a1, 32, v);
-            uint32_t r[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(v[j]);
-            if (tma && EK != EPI_RESID_F32) tma_store_tile(stg_s, lane, r, tmf, gcol0 + 32, row0);
-            else store_tile128<EK == EPI_RESID_F32>(stg_s, lane, r, ob + 128, rb + 128, ldb, row0, M);
-        }
-    } else if (EK == EPI_GLU_F32) {
-        uint32_t r[32];
-        {
-            float v[32];
-            rowmath(a0, 0, v);
-#pragma unroll
-            for (int k = 0; k < 16; ++k) r[k] = __float_as_uint(v[2 * k] * fast_sigmoid(v[2 * k + 1]));
-        }
-        {
-            float v[32];
-            rowmath(a1, 32, v);
-#pragma unroll
-            for (int k = 0; k < 16; ++k) r[16 + k] = __float_as_uint(v[2 * k] * fast_sigmoid(v[2 * k + 1]));
-        }
-        if (tl) tl[5] = tl[6] = clock64();
-        if (tma) tma_store_tile(stg_s, lane, r, tm0, gcol0 >> 1, row0);
-        else store_tile128<false>(stg_s, lane, r, reinterpret_cast<uint8_t *>(epi.out_f32 + (gcol0 >> 1)), nullptr, (size_t)epi.ldo * 4, row0, M);
-    } else {
-        // bf16 hi / lo planes: 64 columns = 128 B per lane and plane  (EPI_QKV_ACT: the k | v columns, planes [M, N - qcols])
-        const size_t ldb = (size_t)epi.ldo * 2;
-        const int col = (EK == EPI_QKV_ACT) ? gcol0 - epi.qcols : gcol0;
-        uint32_t hi[32], lo[32];
-        {
-            float v[32];
-            rowmath(a0, 0, v);
-#pragma unroll
-            for (int j = 0; j < 32; j += 2) split_pair(v[j], v[j + 1], hi[j >> 1], lo[j >> 1]);
-        }
-        {
-            float v[32];
-            rowmath(a1, 32, v);
-#pragma unroll
-            for (int j = 0; j < 32; j += 2) split_pair(v[j], v[j + 1], hi[16 + (j >> 1)], lo[16 + (j >> 1)]);
-        }
-        if (tl) tl[5] = clock64();
-        if (tma) {
-            tma_store_tile(stg_s, lane, hi, tm0, col, row0);
-            if (tl) tl[6] = clock64();
-            if (epi.act.lo) tma_store_tile(stg_s, lane, lo, tm1, col, row0);
-        } else {
-            store_tile128<false>(stg_s, lane, hi, reinterpret_cast<uint8_t *>(epi.act.hi + col), nullptr, ldb, row0, M);
-            if (tl) tl[6] = clock64();
-            if (epi.act.lo) store_tile128<false>(stg_s, lane, lo, reinterpret_cast<uint8_t *>(epi.act.lo + col), nullptr, ldb, row0, M);
-        }
-    }
-}
-
-constexpr int EPI_WARPS = 8;                    // two per TMEM lane quarter, each half of the columns
-constexpr int TC_THREADS_P = 64 + EPI_WARPS * 32;
-
-template <int BN, int NPASS>
+template <int BN, int NPASS, bool LN = false>
 struct TcCfg {
     static constexpr int A_BYTES = BM * BK * 2;                 // one plane, 16 KB
     static constexpr int W_BYTES = BN * BK * 2;
     static constexpr int PLANES = (NPASS == 3) ? 2 : 1;
     static constexpr int STAGE_BYTES = PLANES * (A_BYTES + W_BYTES);
-    static constexpr int STG_BYTES = EPI_WARPS * STGW_BYTES;    // epilogue staging: one 32 x 128 B tile per warp
-    static constexpr int AVAIL = 227 * 1024 - STG_BYTES - 1024 - 256;
+    static constexpr int STAT_BYTES = LN ? 4 * BM * 4 * 4 : 0;  // fused LayerNorm: 4 exchanges x 128 rows x 4 CTAs (fp32)
+    static constexpr int AVAIL = 227 * 1024 - STAT_BYTES - 1024 - 256;
     static constexpr int STAGES = AVAIL / STAGE_BYTES > 8 ? 8 : AVAIL / STAGE_BYTES;
-    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + STG_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-    static constexpr int TMEM_COLS = 2 * BN;                    // double-buffered accumulator
-    static_assert(STG_BYTES >= EPI_WARPS * 32 * STG_LD * 4, "staging also serves the 16-column path");
+    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + STAT_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+    static_assert(STAGES >= 2, "pipeline depth");
 };
 
-// Persistent: grid = min(#tiles, #SMs); CTA c takes tiles c, c+grid, ...  (n-tile fastest so
-// concurrently running CTAs share the same A rows through L2).  The accumulator is double
-// buffered in TMEM so the epilogue of tile i overlaps the MMAs of tile i+1.
-// CL > 1 (gemm_tc_cl_kernel): thread-block clusters of CL CTAs along N.  The CL CTAs of a cluster work on the SAME 128-row
-// block and on adjacent column tiles, so the A tile of a k-block is identical for all of them: each CTA fetches 128 / CL of
-// its rows (tmA_* then have a 128 / CL-row box) and TMA-MULTICASTS the slice into the stage of every CTA of the cluster.  A
-// stage is then written by all CTAs, so its "empty" barrier collects one tcgen05.commit (multicast) from each of them.
-// Why: with three 64 KB stages a CTA has 192 KB of operands in flight; at the ~1.5 us L2 latency of a loaded chip that is
-// 69 B/clk/SM (Little's law) against the 71 B/clk/SM that back-to-back UMMAs consume -- any extra latency (result stores
-// sharing the L2) stalls the MMA warp (measured: 7.3k -> 9.4k cycles per tile).  Multicast cuts the bytes a CTA has to pull
-// per k-block from 64 KB to 32 + 32 / CL KB, i.e. the same bytes in flight cover 1.33x (CL = 2) / 1.6x (CL = 4) the latency.
-template <int BN, int NPASS, int EK, int CL>
-__device__ __forceinline__ void gemm_tc_body(const CUtensorMap &tmA_hi, const CUtensorMap &tmA_lo, const CUtensorMap &tmW_hi, const CUtensorMap &tmW_lo,
-                                             int M, int N, int K, const EpiParams &epi, int dbg, const CUtensorMap &tmO0, const CUtensorMap &tmO1,
-                                             const CUtensorMap &tmO2) {
-    using C = TcCfg<BN, NPASS>;
+constexpr int LN_CL = 4;        // fused LayerNorm: one cluster of 4 CTAs x 128 columns = one 512-wide row block
+
+// Epilogue of one consumer warpgroup: its 64 x BN accumulator slab, rows row0.., columns n0...  Lanes t and t ^ 1 swap
+// the row-(r + 8) pair of one and the row-r pair of the other, so every lane holds 4 consecutive columns of one row --
+// the unit every epilogue kind works on (GLU pairs stay in-thread, vector stores).
+template <int BN, int EK>
+__device__ __forceinline__ void epilogue_regs(const float (&d)[BN / 2], const EpiParams &epi_param, int row0, int n0, int M, int N, int lane) {
+    const EpiParams epi = epi_param;
+    const int q = lane & 3;
+    const int row = row0 + (lane >> 2) + ((q & 1) ? 8 : 0);
+    const bool vec_ok = ((epi.ldo & 3) == 0) && ((N & 3) == 0);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+        // even lane: keeps its row-r pair, receives the partner's row-r pair; odd lane: the row-(r + 8) pairs
+        const float s0 = (q & 1) ? d[4 * j] : d[4 * j + 2], s1 = (q & 1) ? d[4 * j + 1] : d[4 * j + 3];
+        const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+        if (row >= M) continue;
+        float4 v = (q & 1) ? make_float4(r0, r1, d[4 * j + 2], d[4 * j + 3]) : make_float4(d[4 * j], d[4 * j + 1], r0, r1);
+        const int col = n0 + 8 * j + 4 * (q >> 1);
+        if (vec_ok && col + 4 <= N) {
+            float4 b = make_float4(0.f, 0.f, 0.f, 0.f), r = b;
+            if (epi.bias) b = __ldg(reinterpret_cast<const float4 *>(epi.bias + col));
+            if (EK == EPI_RESID_F32) r = *reinterpret_cast<const float4 *>(epi.resid + (size_t)row * epi.ldo + col);
+            epi_store<EK>(epi, row, col, epi_math<EK>(v, b, r, epi.alpha));
+        } else {
+            epilogue4(epi_param, row, col, N, v);
+        }
+    }
+}
+
+// keeps the compiler from moving accesses of the accumulator registers across wgmma issue / wait
+template <int N>
+__device__ __forceinline__ void fence_operands(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// Sum over the cluster of one per-row partial: lane `writer` of each row stores its CTA's partial into slot `rank` of the
+// row in every CTA's buffer, one cluster barrier, then every CTA adds the four slots in the same order.  Every thread of
+// every CTA must call it the same number of times (the barrier).
+__device__ __forceinline__ float cluster_row_sum(float part, float *buf, int lrow, bool writer, uint32_t rank) {
+    if (writer) {
+        const uint32_t a = smem_u32(buf + lrow * LN_CL + rank);
+#pragma unroll
+        for (uint32_t r = 0; r < (uint32_t)LN_CL; ++r) st_cluster_f32(mapa_rank(a, r), part);
+    }
+    cluster_sync();
+    const float4 v = *reinterpret_cast<const float4 *>(buf + lrow * LN_CL);
+    return ((v.x + v.y) + v.z) + v.w;
+}
+
+// Fused LayerNorm epilogue of one consumer warpgroup (BN = 128 columns of a 512-wide row; the row lives in the 4 CTAs of
+// the cluster).  Two passes per LayerNorm like layernorm_kernel: mean, then the centred second moment.
+__device__ __forceinline__ void epilogue_ln(const float (&d)[64], const LnEpi &ep, int row0, int lrow0, int n0, int M, int N, int lane,
+                                            float *stat, uint32_t rank) {
+    const int q = lane & 3;
+    const int row = row0 + (lane >> 2) + ((q & 1) ? 8 : 0), lrow = lrow0 + (lane >> 2) + ((q & 1) ? 8 : 0);
+    const bool writer = (q >> 1) == 0, live = row < M;
+    float x[64];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        const float s0 = (q & 1) ? d[4 * j] : d[4 * j + 2], s1 = (q & 1) ? d[4 * j + 1] : d[4 * j + 3];
+        const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+        const float4 v = (q & 1) ? make_float4(r0, r1, d[4 * j + 2], d[4 * j + 3]) : make_float4(d[4 * j], d[4 * j + 1], r0, r1);
+        const int col = n0 + 8 * j + 4 * (q >> 1);
+        float4 b = make_float4(0.f, 0.f, 0.f, 0.f), r = b;
+        if (ep.bias) b = __ldg(reinterpret_cast<const float4 *>(ep.bias + col));
+        if (ep.resid && live) r = *reinterpret_cast<const float4 *>(ep.resid + (size_t)row * N + col);
+        x[4 * j] = r.x + ep.alpha * (v.x + b.x);
+        x[4 * j + 1] = r.y + ep.alpha * (v.y + b.y);
+        x[4 * j + 2] = r.z + ep.alpha * (v.z + b.z);
+        x[4 * j + 3] = r.w + ep.alpha * (v.w + b.w);
+    }
+    auto store_f32 = [&]() {
+        if (!live || !ep.out_f32) return;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+            *reinterpret_cast<float4 *>(ep.out_f32 + (size_t)row * N + n0 + 8 * j + 4 * (q >> 1)) =
+                make_float4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
+    };
+    auto layernorm = [&](const float *w, const float *bb, float *buf) {
+        float s = 0.f;
+#pragma unroll
+        for (int i = 0; i < 64; ++i) s += x[i];
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        const float mean = cluster_row_sum(s, buf, lrow, writer, rank) / (float)N;
+        float c = 0.f;
+#pragma unroll
+        for (int i = 0; i < 64; ++i) c += (x[i] - mean) * (x[i] - mean);
+        c += __shfl_xor_sync(0xffffffffu, c, 2);
+        const float rstd = rsqrtf(cluster_row_sum(c, buf + BM * LN_CL, lrow, writer, rank) / (float)N + ep.eps);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const int col = n0 + 8 * j + 4 * (q >> 1);
+            const float4 g = __ldg(reinterpret_cast<const float4 *>(w + col)), o = __ldg(reinterpret_cast<const float4 *>(bb + col));
+            x[4 * j] = (x[4 * j] - mean) * rstd * g.x + o.x;
+            x[4 * j + 1] = (x[4 * j + 1] - mean) * rstd * g.y + o.y;
+            x[4 * j + 2] = (x[4 * j + 2] - mean) * rstd * g.z + o.z;
+            x[4 * j + 3] = (x[4 * j + 3] - mean) * rstd * g.w + o.w;
+        }
+    };
+    if (!ep.out_ln1) store_f32();
+    layernorm(ep.ln1_w, ep.ln1_b, stat);
+    if (ep.out_ln1) store_f32();
+    if (ep.ln2_w) layernorm(ep.ln2_w, ep.ln2_b, stat + 2 * BM * LN_CL);
+    if (live) {
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+            store_act4(ep.planes, (size_t)row * N + n0 + 8 * j + 4 * (q >> 1), make_float4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]));
+    }
+}
+
+// The kernel body, shared by the three kernels below.
+// CL > 1: thread-block clusters of CL CTAs along N.  The CL CTAs of a cluster work on the SAME 128-row block and on adjacent
+// column tiles, so the A tile of a k-block is the same for all of them.  MC: each CTA fetches 128 / CL of its rows (tmA_*
+// then have a 128 / CL-row box) and TMA-multicasts the slice into the stage of every CTA of the cluster; a stage is then
+// written by all CTAs, so its "empty" barrier collects the arrivals of the consumer warps of all of them.
+// LN: the fused LayerNorm epilogue (CL = 4, N = 512, one unit per cluster: grid = 4 x row blocks).
+template <int BN, int NPASS, int EK, int CL, bool MC, bool LN>
+__device__ __forceinline__ void gemm_tc_body(const CUtensorMap &tmA_hi, const CUtensorMap &tmA_lo, const CUtensorMap &tmW_hi,
+                                             const CUtensorMap &tmW_lo, int M, int N, int K, const EpiParams &epi, const LnEpi &lnp) {
+    using C = TcCfg<BN, NPASS, LN>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    float *staging = reinterpret_cast<float *>(tiles + (size_t)C::STAGES * C::STAGE_BYTES);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(reinterpret_cast<uint8_t *>(staging) + C::STG_BYTES);
-    uint64_t *full = bars, *empty = bars + C::STAGES, *acc_full = bars + 2 * C::STAGES, *acc_empty = acc_full + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
+    float *stat = reinterpret_cast<float *>(tiles + (size_t)C::STAGES * C::STAGE_BYTES);
+    uint64_t *full = reinterpret_cast<uint64_t *>(tiles + (size_t)C::STAGES * C::STAGE_BYTES + C::STAT_BYTES), *empty = full + C::STAGES;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
     const int nkb = K / BK;
     const int tiles_n = (N + BN - 1) / BN, tiles_m = (M + BM - 1) / BM;
-    // work units of a CTA: tile = first + i * step; CL > 1: the cluster walks (row block, group of CL column tiles) and this
-    // CTA takes column tile `rank` of the group (tiles_n % CL == 0, checked by the launcher)
-    const int rank = CL > 1 ? (int)cluster_ctarank() : 0;
-    const int first_unit = CL > 1 ? (int)(blockIdx.x / CL) : (int)blockIdx.x, unit_step = CL > 1 ? (int)(gridDim.x / CL) : (int)gridDim.x;
-    const int num_tiles = CL > 1 ? (tiles_n / CL) * tiles_m : tiles_n * tiles_m;      // units
-    auto unit_m0 = [&](int u) { return CL > 1 ? (u / (tiles_n / CL)) * BM : (u / tiles_n) * BM; };
-    auto unit_n0 = [&](int u) { return CL > 1 ? ((u % (tiles_n / CL)) * CL + rank) * BN : (u % tiles_n) * BN; };
+    // work units: the cluster walks (row block, group of CL column tiles); this CTA takes column tile `rank` of the group
+    // (tiles_n % CL == 0, checked by the launchers)
+    const uint32_t rank = CL > 1 ? cluster_ctarank() : 0u;
+    const int group_n = tiles_n / CL, num_units = group_n * tiles_m;
+    const int first = (int)blockIdx.x / CL, step = (int)gridDim.x / CL;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < C::STAGES; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], CL);
-        }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(&acc_full[b], 1);
-            mbar_init(&acc_empty[b], EPI_WARPS);
+            mbar_init(&empty[s], CONSUMER_WARPS * (MC ? CL : 1));
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(C::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
-    if (CL > 1) cluster_sync();      // every CTA's barriers exist before a peer multicasts into this CTA
+    if (CL > 1) cluster_sync();      // every CTA's barriers exist before a peer multicasts into it / arrives on them
     else __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_wait();      // barriers, TMEM and the role split are set up while the previous grid drains; now its results are visible
+    pdl_wait();      // barriers are set up while the previous grid drains; now its results are visible
     pdl_trigger();
 
-    if (warp == 0) {
+    if (wg == 0) {
         // ===================== TMA producer =====================
-        if (elect_one()) {
-            uint32_t it = 0;   // global k-block counter across tiles
-            const uint64_t ld_policy = g_l2_hint_mode == 1 ? L2_EVICT_NORMAL : L2_EVICT_LAST;
-            for (int tile = first_unit; tile < num_tiles; tile += unit_step) {
-                const int m0 = unit_m0(tile), n0 = unit_n0(tile);
+        if (warp == 0 && elect_one()) {
+            uint32_t it = 0;   // global k-block counter across units
+            for (int u = first; u < num_units; u += step) {
+                const int m0 = (u / group_n) * BM, n0 = ((u % group_n) * CL + (int)rank) * BN;
                 for (int kb = 0; kb < nkb; ++kb, ++it) {
                     const int s = it % C::STAGES;
                     const uint32_t ph = (it / C::STAGES) & 1;
                     mbar_wait(&empty[s], ph ^ 1);
                     uint8_t *st = tiles + (size_t)s * C::STAGE_BYTES;
-                    if (dbg & 2) { mbar_arrive(&full[s]); continue; }      // measurement aid: MMAs on stale smem, no loads
                     mbar_expect_tx(&full[s], C::STAGE_BYTES);
-                    if (CL > 1) {       // this CTA's slice of the A rows, into the stage of every CTA of the cluster
+                    if (MC) {       // this CTA's slice of the A rows, into the stage of every CTA of the cluster
                         constexpr int SL = BM / CL, SLB = SL * BK * 2;
                         constexpr uint16_t mask = (uint16_t)((1u << CL) - 1u);
-                        tma_load_2d_mcast(st + rank * SLB, &tmA_hi, &full[s], kb * BK, m0 + rank * SL, mask, ld_policy);
-                        if (NPASS == 3) tma_load_2d_mcast(st + C::A_BYTES + C::W_BYTES + rank * SLB, &tmA_lo, &full[s], kb * BK, m0 + rank * SL, mask, ld_policy);
+                        tma_load_2d_mcast(st + rank * SLB, &tmA_hi, &full[s], kb * BK, m0 + (int)rank * SL, mask);
+                        if (NPASS == 3) tma_load_2d_mcast(st + C::A_BYTES + C::W_BYTES + rank * SLB, &tmA_lo, &full[s], kb * BK, m0 + (int)rank * SL, mask);
                     } else {
-                        tma_load_2d(st, &tmA_hi, &full[s], kb * BK, m0, ld_policy);
-                        if (NPASS == 3) tma_load_2d(st + C::A_BYTES + C::W_BYTES, &tmA_lo, &full[s], kb * BK, m0, ld_policy);
+                        tma_load_2d(st, &tmA_hi, &full[s], kb * BK, m0);
+                        if (NPASS == 3) tma_load_2d(st + C::A_BYTES + C::W_BYTES, &tmA_lo, &full[s], kb * BK, m0);
                     }
-                    tma_load_2d(st + C::A_BYTES, &tmW_hi, &full[s], kb * BK, n0, ld_policy);
-                    if (NPASS == 3) tma_load_2d(st + 2 * C::A_BYTES + C::W_BYTES, &tmW_lo, &full[s], kb * BK, n0, ld_policy);
+                    tma_load_2d(st + C::A_BYTES, &tmW_hi, &full[s], kb * BK, n0);
+                    if (NPASS == 3) tma_load_2d(st + 2 * C::A_BYTES + C::W_BYTES, &tmW_lo, &full[s], kb * BK, n0);
                 }
             }
             pdl_trigger_late();     // every operand load of this CTA has been issued
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            constexpr uint32_t idesc = umma_idesc_bf16(BM, BN);
-            uint32_t it = 0, tcount = 0;
-            for (int tile = first_unit; tile < num_tiles; tile += unit_step, ++tcount) {
-                const uint32_t buf = tcount & 1, aph = (tcount >> 1) & 1;
-                mbar_wait(&acc_empty[buf], aph ^ 1);      // epilogue has drained this accumulator
-                tcgen05_fence_after();
-                if ((dbg & 32) && blockIdx.x == 0 && tcount < 64) g_timeline[tcount][0] = clock64();
-                const uint32_t tmem_d = tmem_base + buf * BN;
-                for (int kb = 0; kb < nkb; ++kb, ++it) {
-                    const int s = it % C::STAGES;
-                    const uint32_t ph = (it / C::STAGES) & 1;
-                    mbar_wait(&full[s], ph);
-                    tcgen05_fence_after();
-                    const uint32_t st = smem_u32(tiles + (size_t)s * C::STAGE_BYTES);
-                    const uint64_t a_hi = umma_desc_sw128(st), w_hi = umma_desc_sw128(st + C::A_BYTES);
-                    const uint64_t a_lo = umma_desc_sw128(st + C::A_BYTES + C::W_BYTES);
-                    const uint64_t w_lo = umma_desc_sw128(st + 2 * C::A_BYTES + C::W_BYTES);
-#pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; ++k) {
-                        const uint64_t koff = (uint64_t)((k * UMMA_K * 2) >> 4);   // 32 B per K step, encoded >>4
-                        umma_bf16(tmem_d, a_hi + koff, w_hi + koff, idesc, (kb | k) != 0);
-                        if (NPASS == 3) {
-                            umma_bf16(tmem_d, a_hi + koff, w_lo + koff, idesc, 1);
-                            umma_bf16(tmem_d, a_lo + koff, w_hi + koff, idesc, 1);
-                        }
-                    }
-                    if (CL > 1) umma_commit_mcast(&empty[s], (uint16_t)((1u << CL) - 1u));   // ... in every CTA of the cluster (they all write it)
-                    else umma_commit(&empty[s]);     // frees the stage when these MMAs retire
-                }
-                umma_commit(&acc_full[buf]);         // accumulator of this tile complete
-                if ((dbg & 32) && blockIdx.x == 0 && tcount < 64) g_timeline[tcount][1] = clock64();
-            }
+        __syncwarp();                // the elected lane rejoins its warp before the .aligned cluster barriers below
+        if (LN) {                    // the producer warpgroup takes part in the epilogue's cluster barriers
+            const int n_sync = lnp.ln2_w ? 4 : 2;
+            for (int i = 0; i < n_sync; ++i) cluster_sync();
         }
     } else {
-        // ===================== epilogue (warps 2..9) =====================
-        const int ew = warp - 2;
-        const int q = warp & 3;                      // TMEM lane quarter this warp may access
-        const int half = ew >> 2;                    // which half of the BN columns
-        const uint32_t stg_s = smem_u32(staging) + (uint32_t)ew * STGW_BYTES;   // explicit .shared accesses
-        uint32_t tcount = 0;
-        const bool probe = dbg && blockIdx.x == 0 && threadIdx.x == 64;
-        long long pc0 = 0;
-        unsigned long long pg0 = 0;
-        if (probe) { pc0 = clock64(); pg0 = globaltimer_ns(); }
-        for (int tile = first_unit; tile < num_tiles; tile += unit_step, ++tcount) {
-            const int m0 = unit_m0(tile), n0 = unit_n0(tile);
-            const uint32_t buf = tcount & 1, aph = (tcount >> 1) & 1;
-            mbar_wait(&acc_full[buf], aph);
-            tcgen05_fence_after();
-            if ((dbg & 32) && blockIdx.x == 0 && threadIdx.x == 64 && tcount < 64) g_timeline[tcount][2] = clock64();
-            const uint32_t taddr = tmem_base + buf * BN + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * (BN / 2));
-            if (dbg & 1) {                           // measurement aid: drain nothing, release at once
-                tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&acc_empty[buf]);
-                continue;
+        // ===================== consumers: wgmma + epilogue =====================
+        const int cw = wg - 1;                              // row half of the tile
+        const uint32_t a_off = (uint32_t)cw * 64u * 128u;   // 64 rows of 128 B
+        auto release = [&](int s) {                         // this warp has finished reading stage s
+            __syncwarp();
+            if (lane == 0) {
+                if (MC) {
+                    const uint32_t a = smem_u32(&empty[s]);
+#pragma unroll
+                    for (uint32_t r = 0; r < (uint32_t)CL; ++r) mbar_arrive_cluster(mapa_rank(a, r));
+                } else {
+                    mbar_arrive(&empty[s]);
+                }
             }
-            auto release = [&]() {
-                tcgen05_fence_before();              // last TMEM read of this tile has landed: release the buffer
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&acc_empty[buf]);
-            };
-            if (BN == 128 && !(dbg & 64) && wide_ok<EK>(epi, n0 + half * 64, N)) {
-                long long *tl = ((dbg & 32) && blockIdx.x == 0 && threadIdx.x == 64 && tcount < 64) ? g_timeline[tcount] : nullptr;
-                epilogue_slab64<EK>(taddr, stg_s, m0 + q * 32, n0 + half * 64, M, epi, lane, release, true, &tmO0, &tmO1, &tmO2, tl);
-            } else {
-                if (epi.tma_out) stg_acquire(lane);
-                epilogue_slab<BN / 2, EK>(taddr, stg_s, m0 + q * 32, n0 + half * (BN / 2), M, N, epi, lane, release, dbg);
+        };
+        uint32_t it = 0;
+        for (int u = first; u < num_units; u += step) {
+            const int m0 = (u / group_n) * BM, n0 = ((u % group_n) * CL + (int)rank) * BN;
+            float d[BN / 2];
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+            fence_operands(d);
+            int prev_s = -1;
+            for (int kb = 0; kb < nkb; ++kb, ++it) {
+                const int s = it % C::STAGES;
+                const uint32_t ph = (it / C::STAGES) & 1;
+                mbar_wait(&full[s], ph);
+                const uint32_t st = smem_u32(tiles + (size_t)s * C::STAGE_BYTES);
+                const uint64_t a_hi = wgmma_desc_sw128(st + a_off), w_hi = wgmma_desc_sw128(st + C::A_BYTES);
+                const uint64_t a_lo = wgmma_desc_sw128(st + C::A_BYTES + C::W_BYTES + a_off);
+                const uint64_t w_lo = wgmma_desc_sw128(st + 2 * C::A_BYTES + C::W_BYTES);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / WGMMA_K; ++k) {
+                    const uint64_t koff = (uint64_t)((k * WGMMA_K * 2) >> 4);   // 32 B per K step, encoded >> 4
+                    wgmma_bf16<BN>(d, a_hi + koff, w_hi + koff);
+                    if (NPASS == 3) {
+                        wgmma_bf16<BN>(d, a_hi + koff, w_lo + koff);
+                        wgmma_bf16<BN>(d, a_lo + koff, w_hi + koff);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<1>();                            // the group of the previous k-block has retired
+                if (prev_s >= 0) release(prev_s);
+                prev_s = s;
             }
-            if ((dbg & 32) && blockIdx.x == 0 && threadIdx.x == 64 && tcount < 64) g_timeline[tcount][3] = clock64();
+            wgmma_wait<0>();
+            fence_operands(d);
+            if (prev_s >= 0) release(prev_s);
+            const int lrow0 = cw * 64 + (warp & 3) * 16;
+            if constexpr (LN) epilogue_ln(d, lnp, m0 + lrow0, lrow0, n0, M, N, lane, stat, rank);
+            else epilogue_regs<BN, EK>(d, epi, m0 + lrow0, n0, M, N, lane);
         }
-        if (probe) { g_clk_probe[0] = (unsigned long long)(clock64() - pc0); g_clk_probe[1] = globaltimer_ns() - pg0; }
-        if (epi.tma_out && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // this warp's TMA stores have completed
     }
-    tcgen05_fence_before();
-    if (CL > 1) cluster_sync();      // nobody leaves while a peer may still multicast into it / signal its barriers
-    else __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(C::TMEM_COLS) : "memory");
-    }
+    if (CL > 1) cluster_sync();      // nobody leaves while a peer may still multicast into it / arrive on its barriers
 }
 
 template <int BN, int NPASS, int EK>
-__global__ void __launch_bounds__(TC_THREADS_P, 1)
+__global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, int M, int N,
-               int K, const __grid_constant__ EpiParams epi, int dbg, const __grid_constant__ CUtensorMap tmO0,
-               const __grid_constant__ CUtensorMap tmO1, const __grid_constant__ CUtensorMap tmO2) {
-    gemm_tc_body<BN, NPASS, EK, 1>(tmA_hi, tmA_lo, tmW_hi, tmW_lo, M, N, K, epi, dbg, tmO0, tmO1, tmO2);
+               int K, const __grid_constant__ EpiParams epi) {
+    gemm_tc_body<BN, NPASS, EK, 1, false, false>(tmA_hi, tmA_lo, tmW_hi, tmW_lo, M, N, K, epi, LnEpi());
 }
 
-// clusters of CL CTAs along N with the A tile multicast (see gemm_tc_body); 128-column tiles only
+// clusters of CL CTAs along N with the A tile multicast; 128-column tiles only
 template <int NPASS, int EK, int CL>
-__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(TC_THREADS_P, 1)
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(TC_THREADS, 1)
 gemm_tc_cl_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                   const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, int M, int N,
-                  int K, const __grid_constant__ EpiParams epi, int dbg, const __grid_constant__ CUtensorMap tmO0,
-                  const __grid_constant__ CUtensorMap tmO1, const __grid_constant__ CUtensorMap tmO2) {
-    gemm_tc_body<128, NPASS, EK, CL>(tmA_hi, tmA_lo, tmW_hi, tmW_lo, M, N, K, epi, dbg, tmO0, tmO1, tmO2);
+                  int K, const __grid_constant__ EpiParams epi) {
+    gemm_tc_body<128, NPASS, EK, CL, true, false>(tmA_hi, tmA_lo, tmW_hi, tmW_lo, M, N, K, epi, LnEpi());
 }
 
-// =====================================================================================
-// 2-CTA variant (cta_group::2): a CTA PAIR (cluster 2x1x1, the two SMs of a TPC) computes a
-// 256 x 256 output tile with one UMMA M=256 x N=256 x K=16 per instruction.  Each CTA stages only
-// ITS half of both operands (its 128 rows of A, its 128 rows of W) -- the same 64 KB per k-block
-// as the 1-CTA kernel -- but the pair produces 4x the outputs, so the L2->SM operand traffic per
-// flop is halved (the 1-CTA kernel is L2-bandwidth-bound with the 4 split planes: 85 B/cycle/SM
-// needed vs ~43 available).  Roles per CTA as above; only the leader (cluster rank 0) issues
-// MMAs; the peer's TMA loads complete on the LEADER's full barrier; tcgen05.commit multicasts the
-// "stage free" / "accumulator ready" arrivals to both CTAs; each CTA drains its own 128 TMEM
-// lanes; the leader's acc_empty barrier collects the arrivals of both epilogues.
-constexpr int BN2 = 256;
-
-__device__ __forceinline__ void tma_load_2d_2sm(void *smem_dst, const CUtensorMap *tm, uint32_t leader_bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(leader_bar), "r"(c0), "r"(c1)
-        : "memory");
+// residual GEMM + fused LayerNorm(s): clusters of 4 CTAs = one 512-column row block; MC = A tile multicast
+template <int NPASS, bool MC>
+__global__ void __cluster_dims__(LN_CL, 1, 1) __launch_bounds__(TC_THREADS, 1)
+gemm_tc_ln_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
+                  const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, int M, int N,
+                  int K, const __grid_constant__ LnEpi lnp) {
+    gemm_tc_body<128, NPASS, EPI_BIAS_F32, LN_CL, MC, true>(tmA_hi, tmA_lo, tmW_hi, tmW_lo, M, N, K, EpiParams(), lnp);
 }
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint64_t *bar) {   // arrives on `bar` in BOTH CTAs of the pair
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-                 : "memory");
-}
-
-template <int NPASS>
-struct Tc2Cfg {
-    static constexpr int A_BYTES = BM * BK * 2;                 // this CTA's 128 rows of A, one plane
-    static constexpr int W_BYTES = (BN2 / 2) * BK * 2;          // this CTA's 128 rows of W, one plane
-    static constexpr int PLANES = (NPASS == 3) ? 2 : 1;
-    static constexpr int STAGE_BYTES = PLANES * (A_BYTES + W_BYTES);
-    static constexpr int STG_BYTES = EPI_WARPS * STGW_BYTES;
-    static constexpr int AVAIL = 227 * 1024 - STG_BYTES - 1024 - 256;
-    static constexpr int STAGES = AVAIL / STAGE_BYTES > 8 ? 8 : AVAIL / STAGE_BYTES;
-    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + STG_BYTES + 1024 + 256;
-    static constexpr int TMEM_COLS = 2 * BN2;                   // 512: double-buffered 256-column accumulator
-};
-
-template <int NPASS, int EK>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS_P, 1)
-gemm_tc2_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, int M, int N,
-                int K, const __grid_constant__ EpiParams epi, int dbg, const __grid_constant__ CUtensorMap tmO0,
-                const __grid_constant__ CUtensorMap tmO1, const __grid_constant__ CUtensorMap tmO2) {
-    using C = Tc2Cfg<NPASS>;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    float *staging = reinterpret_cast<float *>(tiles + (size_t)C::STAGES * C::STAGE_BYTES);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(reinterpret_cast<uint8_t *>(staging) + C::STG_BYTES);
-    uint64_t *full = bars, *empty = bars + C::STAGES, *acc_full = bars + 2 * C::STAGES, *acc_empty = acc_full + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const int nkb = K / BK;
-    const int tiles_n = (N + BN2 - 1) / BN2, tiles_m = (M + 2 * BM - 1) / (2 * BM);
-    const int num_tiles = tiles_n * tiles_m;
-    const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < C::STAGES; ++s) {
-            mbar_init(&full[s], 2);              // leader producer (arrive + expect_tx) + peer producer (remote arrive)
-            mbar_init(&empty[s], 1);             // multicast tcgen05.commit from the leader
-        }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(&acc_full[b], 1);          // multicast tcgen05.commit from the leader
-            mbar_init(&acc_empty[b], 2 * EPI_WARPS);   // both CTAs' epilogue warps (leader's copy is the one used)
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {   // both CTAs of the pair allocate (same warp id, same columns)
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(C::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
-    cluster_sync();                              // barriers of both CTAs initialised before any remote arrive
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_wait();      // barriers, TMEM and the role split are set up while the previous grid drains; now its results are visible
-    pdl_trigger();
-
-    if (warp == 0) {
-        // ===================== TMA producer (both CTAs) =====================
-        if (elect_one()) {
-            uint32_t it = 0;
-            for (int tile = pair; tile < num_tiles; tile += npairs) {
-                const int m0 = (tile / tiles_n) * (2 * BM) + (int)rank * BM;
-                const int n0 = (tile % tiles_n) * BN2 + (int)rank * (BN2 / 2);
-                for (int kb = 0; kb < nkb; ++kb, ++it) {
-                    const int s = it % C::STAGES;
-                    const uint32_t ph = (it / C::STAGES) & 1;
-                    mbar_wait(&empty[s], ph ^ 1);
-                    uint8_t *st = tiles + (size_t)s * C::STAGE_BYTES;
-                    const uint32_t lbar = mapa_rank(smem_u32(&full[s]), 0);   // the leader's full barrier
-                    if (dbg & 2) { mbar_arrive_cluster(lbar); continue; }     // measurement aid: no loads
-                    if (leader) mbar_expect_tx(&full[s], 2 * C::STAGE_BYTES);
-                    else mbar_arrive_cluster(lbar);
-                    tma_load_2d_2sm(st, &tmA_hi, lbar, kb * BK, m0);
-                    tma_load_2d_2sm(st + C::A_BYTES, &tmW_hi, lbar, kb * BK, n0);
-                    if (NPASS == 3) {
-                        tma_load_2d_2sm(st + C::A_BYTES + C::W_BYTES, &tmA_lo, lbar, kb * BK, m0);
-                        tma_load_2d_2sm(st + 2 * C::A_BYTES + C::W_BYTES, &tmW_lo, lbar, kb * BK, n0);
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (leader CTA only) =====================
-        if (leader && elect_one()) {
-            constexpr uint32_t idesc = umma_idesc_bf16(2 * BM, BN2);
-            uint32_t it = 0, tcount = 0;
-            for (int tile = pair; tile < num_tiles; tile += npairs, ++tcount) {
-                const uint32_t buf = tcount & 1, aph = (tcount >> 1) & 1;
-                mbar_wait(&acc_empty[buf], aph ^ 1);
-                tcgen05_fence_after();
-                if ((dbg & 32) && blockIdx.x == 0 && tcount < 64) g_timeline[tcount][0] = clock64();
-                const uint32_t tmem_d = tmem_base + buf * BN2;
-                for (int kb = 0; kb < nkb; ++kb, ++it) {
-                    const int s = it % C::STAGES;
-                    const uint32_t ph = (it / C::STAGES) & 1;
-                    mbar_wait(&full[s], ph);
-                    tcgen05_fence_after();
-                    const uint32_t st = smem_u32(tiles + (size_t)s * C::STAGE_BYTES);
-                    const uint64_t a_hi = umma_desc_sw128(st), w_hi = umma_desc_sw128(st + C::A_BYTES);
-                    const uint64_t a_lo = umma_desc_sw128(st + C::A_BYTES + C::W_BYTES);
-                    const uint64_t w_lo = umma_desc_sw128(st + 2 * C::A_BYTES + C::W_BYTES);
-#pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; ++k) {
-                        const uint64_t koff = (uint64_t)((k * UMMA_K * 2) >> 4);
-                        umma_bf16_2sm(tmem_d, a_hi + koff, w_hi + koff, idesc, (kb | k) != 0);
-                        if (NPASS == 3) {
-                            umma_bf16_2sm(tmem_d, a_hi + koff, w_lo + koff, idesc, 1);
-                            umma_bf16_2sm(tmem_d, a_lo + koff, w_hi + koff, idesc, 1);
-                        }
-                    }
-                    umma_commit_2sm(&empty[s]);      // frees stage s in both CTAs
-                }
-                umma_commit_2sm(&acc_full[buf]);     // accumulator ready in both CTAs
-                if ((dbg & 32) && blockIdx.x == 0 && tcount < 64) g_timeline[tcount][1] = clock64();
-            }
-        }
-    } else {
-        // ===================== epilogue (warps 2..9 of both CTAs) =====================
-        const int ew = warp - 2;
-        const int q = warp & 3;
-        const int half = ew >> 2;
-        const uint32_t stg_s = smem_u32(staging) + (uint32_t)ew * STGW_BYTES;   // explicit .shared accesses
-        const uint32_t lempty0 = mapa_rank(smem_u32(&acc_empty[0]), 0), lempty1 = mapa_rank(smem_u32(&acc_empty[1]), 0);
-        uint32_t tcount = 0;
-        for (int tile = pair; tile < num_tiles; tile += npairs, ++tcount) {
-            const int m0 = (tile / tiles_n) * (2 * BM) + (int)rank * BM, n0 = (tile % tiles_n) * BN2;
-            const uint32_t buf = tcount & 1, aph = (tcount >> 1) & 1;
-            mbar_wait(&acc_full[buf], aph);
-            tcgen05_fence_after();
-            if ((dbg & 32) && blockIdx.x == 0 && threadIdx.x == 64 && tcount < 64) g_timeline[tcount][2] = clock64();
-            const uint32_t taddr = tmem_base + buf * BN2 + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * (BN2 / 2));
-            if (dbg & 1) {
-                tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(buf ? lempty1 : lempty0);
-                continue;
-            }
-            auto release = [&]() {
-                tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(buf ? lempty1 : lempty0);   // leader's barrier counts both CTAs
-            };
-            const int gc = n0 + half * (BN2 / 2);
-            if (!(dbg & 64) && wide_ok<EK>(epi, gc, N) && wide_ok<EK>(epi, gc + 64, N)) {
-                epilogue_slab64<EK>(taddr, stg_s, m0 + q * 32, gc, M, epi, lane, release, false, &tmO0, &tmO1, &tmO2);
-                epilogue_slab64<EK>(taddr + 64u, stg_s, m0 + q * 32, gc + 64, M, epi, lane, release, true, &tmO0, &tmO1, &tmO2);
-            } else {
-                if (epi.tma_out) stg_acquire(lane);
-                epilogue_slab<BN2 / 2, EK>(taddr, stg_s, m0 + q * 32, gc, M, N, epi, lane, release, dbg);
-            }
-            if ((dbg & 32) && blockIdx.x == 0 && threadIdx.x == 64 && tcount < 64) g_timeline[tcount][3] = clock64();
-        }
-        if (epi.tma_out && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    }
-    tcgen05_fence_before();
-    cluster_sync();                              // nobody leaves (or frees TMEM) while the peer may still signal it
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(C::TMEM_COLS) : "memory");
-    }
-}
-
-int g_dbg = 0;   // PK_GEMM_DBG (measurement aid, tc_set_debug): bit 0 = epilogue releases without draining, bit 1 = no TMA loads
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
@@ -767,6 +327,14 @@ EncodeTiledFn encode_fn() {
     return fn;
 }
 
+int num_sms_cur() {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    static int sms_of[64] = {};
+    if (!sms_of[dev & 63]) cudaDeviceGetAttribute(&sms_of[dev & 63], cudaDevAttrMultiProcessorCount, dev);
+    return sms_of[dev & 63];
+}
+
 template <int BN, int NPASS, int EK>
 cudaError_t launch_k(const TcOperand &A, const TcOperand &W, int M, int N, int K, const EpiParams &epi, cudaStream_t st) {
     using C = TcCfg<BN, NPASS>;
@@ -777,25 +345,27 @@ cudaError_t launch_k(const TcOperand &A, const TcOperand &W, int M, int N, int K
         if (e != cudaSuccess) return e;
         attr = true;
     }
-    int num_sms = 0;
-    {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        static int sms_of[64] = {};
-        if (!sms_of[dev & 63]) cudaDeviceGetAttribute(&sms_of[dev & 63], cudaDevAttrMultiProcessorCount, dev);
-        num_sms = sms_of[dev & 63];
-    }
+    const int num_sms = num_sms_cur();
     const int num_tiles = ((N + BN - 1) / BN) * ((M + BM - 1) / BM);
     dim3 grid(num_tiles < num_sms ? num_tiles : num_sms);
     const CUtensorMap &alo = (NPASS == 3) ? A.lo : A.hi, &wlo = (NPASS == 3) ? W.lo : W.hi;
-    EpiParams ep = epi;
-    const bool tma = ep.tma_out && ep.tm_out0 && BN == 128 && (EK != EPI_QKV_ACT || ep.tm_out2);
-    ep.tma_out = tma ? 1 : 0;
-    const CUtensorMap &o0 = tma ? *static_cast<const CUtensorMap *>(ep.tm_out0) : A.hi;
-    const CUtensorMap &o1 = (tma && ep.tm_out1) ? *static_cast<const CUtensorMap *>(ep.tm_out1) : o0;
-    const CUtensorMap &o2 = (tma && ep.tm_out2) ? *static_cast<const CUtensorMap *>(ep.tm_out2) : o0;
-    launch_pdl(gemm_tc_kernel<BN, NPASS, EK>, dim3(grid), dim3(TC_THREADS_P), C::SMEM, st, A.hi, alo, W.hi, wlo, M, N, K, ep, g_dbg, o0, o1, o2);
+    launch_pdl(gemm_tc_kernel<BN, NPASS, EK>, dim3(grid), dim3(TC_THREADS), C::SMEM, st, A.hi, alo, W.hi, wlo, M, N, K, epi);
     return cudaGetLastError();
+}
+
+template <int BN, int NPASS>
+cudaError_t launch_t(const TcOperand &A, const TcOperand &W, int M, int N, int K, const EpiParams &epi, cudaStream_t st) {
+    switch (epi.kind) {
+    case EPI_BIAS_F32: return launch_k<BN, NPASS, EPI_BIAS_F32>(A, W, M, N, K, epi, st);
+    case EPI_BIAS_RELU_F32: return launch_k<BN, NPASS, EPI_BIAS_RELU_F32>(A, W, M, N, K, epi, st);
+    case EPI_BIAS_RELU_ACT: return launch_k<BN, NPASS, EPI_BIAS_RELU_ACT>(A, W, M, N, K, epi, st);
+    case EPI_BIAS_SILU_ACT: return launch_k<BN, NPASS, EPI_BIAS_SILU_ACT>(A, W, M, N, K, epi, st);
+    case EPI_RESID_F32: return launch_k<BN, NPASS, EPI_RESID_F32>(A, W, M, N, K, epi, st);
+    case EPI_GLU_F32: return launch_k<BN, NPASS, EPI_GLU_F32>(A, W, M, N, K, epi, st);
+    case EPI_BIAS_ACT: return launch_k<BN, NPASS, EPI_BIAS_ACT>(A, W, M, N, K, epi, st);
+    case EPI_QKV_ACT: return launch_k<BN, NPASS, EPI_QKV_ACT>(A, W, M, N, K, epi, st);
+    default: return cudaErrorInvalidValue;
+    }
 }
 
 // cluster / multicast variant: A_sl = the A operand with a 128 / CL-row box
@@ -804,15 +374,15 @@ cudaError_t launch_kcl(const TcOperand &A_sl, const TcOperand &W, int M, int N, 
     using C = TcCfg<128, NPASS>;
     static PerDeviceFlag attr_flag;
     static int max_clusters[64] = {};
-    int dev = 0, num_sms = 0;
+    int dev = 0;
     cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
+    const int num_sms = num_sms_cur();
     if (!attr_flag.cur()) {
         cudaError_t e = cudaFuncSetAttribute(gemm_tc_cl_kernel<NPASS, EK, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
         if (e != cudaSuccess) return e;
         cudaLaunchConfig_t q = {};
         q.gridDim = dim3((unsigned)(num_sms / CL * CL));
-        q.blockDim = dim3(TC_THREADS_P);
+        q.blockDim = dim3(TC_THREADS);
         q.dynamicSmemBytes = C::SMEM;
         int mc = 0;
         if (cudaOccupancyMaxActiveClusters(&mc, gemm_tc_cl_kernel<NPASS, EK, CL>, &q) != cudaSuccess || mc < 1) {
@@ -827,72 +397,21 @@ cudaError_t launch_kcl(const TcOperand &A_sl, const TcOperand &W, int M, int N, 
     if (ncl > num_sms / CL) ncl = num_sms / CL;
     if (ncl > units) ncl = units;
     const CUtensorMap &alo = (NPASS == 3) ? A_sl.lo : A_sl.hi, &wlo = (NPASS == 3) ? W.lo : W.hi;
-    EpiParams ep = epi;
-    const bool tma = ep.tma_out && ep.tm_out0 && (EK != EPI_QKV_ACT || ep.tm_out2);
-    ep.tma_out = tma ? 1 : 0;
-    const CUtensorMap &o0 = tma ? *static_cast<const CUtensorMap *>(ep.tm_out0) : A_sl.hi;
-    const CUtensorMap &o1 = (tma && ep.tm_out1) ? *static_cast<const CUtensorMap *>(ep.tm_out1) : o0;
-    const CUtensorMap &o2 = (tma && ep.tm_out2) ? *static_cast<const CUtensorMap *>(ep.tm_out2) : o0;
-    return launch_pdl(gemm_tc_cl_kernel<NPASS, EK, CL>, dim3((unsigned)(ncl * CL)), dim3(TC_THREADS_P), C::SMEM, st, A_sl.hi, alo, W.hi, wlo, M, N, K, ep, g_dbg, o0, o1,
-                      o2);
+    return launch_pdl(gemm_tc_cl_kernel<NPASS, EK, CL>, dim3((unsigned)(ncl * CL)), dim3(TC_THREADS), C::SMEM, st, A_sl.hi, alo, W.hi, wlo, M, N, K, epi);
 }
 
-template <int NPASS, int EK>
-cudaError_t launch_k2(const TcOperand &A, const TcOperand &W, int M, int N, int K, const EpiParams &epi, cudaStream_t st) {
-    using C = Tc2Cfg<NPASS>;
+template <int NPASS, bool MC>
+cudaError_t launch_ln(const TcOperand &A, const TcOperand &W, int M, int N, int K, const LnEpi &ep, cudaStream_t st) {
+    using C = TcCfg<128, NPASS, true>;
     static PerDeviceFlag attr_flag;
-    bool &attr = attr_flag.cur();
-    if (!attr) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_tc2_kernel<NPASS, EK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
+    if (!attr_flag.cur()) {
+        cudaError_t e = cudaFuncSetAttribute(gemm_tc_ln_kernel<NPASS, MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
         if (e != cudaSuccess) return e;
-        attr = true;
+        attr_flag.cur() = true;
     }
-    int num_sms = 0;
-    {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        static int sms_of[64] = {};
-        if (!sms_of[dev & 63]) cudaDeviceGetAttribute(&sms_of[dev & 63], cudaDevAttrMultiProcessorCount, dev);
-        num_sms = sms_of[dev & 63];
-    }
-    const int num_tiles = ((N + BN2 - 1) / BN2) * ((M + 2 * BM - 1) / (2 * BM));
-    const int pairs = num_tiles < num_sms / 2 ? num_tiles : num_sms / 2;
     const CUtensorMap &alo = (NPASS == 3) ? A.lo : A.hi, &wlo = (NPASS == 3) ? W.lo : W.hi;
-    EpiParams ep = epi;
-    const bool tma = ep.tma_out && ep.tm_out0 && (EK != EPI_QKV_ACT || ep.tm_out2);
-    ep.tma_out = tma ? 1 : 0;
-    const CUtensorMap &o0 = tma ? *static_cast<const CUtensorMap *>(ep.tm_out0) : A.hi;
-    const CUtensorMap &o1 = (tma && ep.tm_out1) ? *static_cast<const CUtensorMap *>(ep.tm_out1) : o0;
-    const CUtensorMap &o2 = (tma && ep.tm_out2) ? *static_cast<const CUtensorMap *>(ep.tm_out2) : o0;
-    launch_pdl(gemm_tc2_kernel<NPASS, EK>, dim3(dim3(2 * pairs)), dim3(TC_THREADS_P), C::SMEM, st, A.hi, alo, W.hi, wlo, M, N, K, ep, g_dbg, o0, o1, o2);
-    return cudaGetLastError();
-}
-
-#define PK_EPI_SWITCH(CALL)                                              \
-    switch (epi.kind) {                                                  \
-    case EPI_BIAS_F32: return CALL(EPI_BIAS_F32);                        \
-    case EPI_BIAS_RELU_F32: return CALL(EPI_BIAS_RELU_F32);              \
-    case EPI_BIAS_RELU_ACT: return CALL(EPI_BIAS_RELU_ACT);              \
-    case EPI_BIAS_SILU_ACT: return CALL(EPI_BIAS_SILU_ACT);              \
-    case EPI_RESID_F32: return CALL(EPI_RESID_F32);                      \
-    case EPI_GLU_F32: return CALL(EPI_GLU_F32);                          \
-    case EPI_BIAS_ACT: return CALL(EPI_BIAS_ACT);                        \
-    case EPI_QKV_ACT: return CALL(EPI_QKV_ACT);                          \
-    default: return cudaErrorInvalidValue;                               \
-    }
-
-template <int BN, int NPASS>
-cudaError_t launch_t(const TcOperand &A, const TcOperand &W, int M, int N, int K, const EpiParams &epi, cudaStream_t st) {
-#define PK_CALL1(EK) launch_k<BN, NPASS, EK>(A, W, M, N, K, epi, st)
-    PK_EPI_SWITCH(PK_CALL1)
-#undef PK_CALL1
-}
-
-template <int NPASS>
-cudaError_t launch_t2(const TcOperand &A, const TcOperand &W, int M, int N, int K, const EpiParams &epi, cudaStream_t st) {
-#define PK_CALL2(EK) launch_k2<NPASS, EK>(A, W, M, N, K, epi, st)
-    PK_EPI_SWITCH(PK_CALL2)
-#undef PK_CALL2
+    const int row_blocks = (M + BM - 1) / BM;
+    return launch_pdl(gemm_tc_ln_kernel<NPASS, MC>, dim3((unsigned)(LN_CL * row_blocks)), dim3(TC_THREADS), C::SMEM, st, A.hi, alo, W.hi, wlo, M, N, K, ep);
 }
 
 }  // namespace
@@ -917,50 +436,14 @@ bool make_tc_operand(TcOperand *out, const bf16 *hi, const bf16 *lo, uint64_t ro
     return true;
 }
 
-bool make_tc_out_map(CUtensorMap *out, const void *ptr, bool is_f32, uint64_t rows, uint64_t ld) {
-    EncodeTiledFn fn = encode_fn();
-    const uint64_t esz = is_f32 ? 4 : 2;
-    if (!fn || !ptr || (reinterpret_cast<uintptr_t>(ptr) & 15) || ((ld * esz) & 15) || rows == 0) return false;
-    const cuuint64_t gdim[2] = {ld, rows};
-    const cuuint64_t gstr[1] = {ld * esz};
-    const cuuint32_t box[2] = {(cuuint32_t)(128 / esz), 32};
-    const cuuint32_t estr[2] = {1, 1};
-    return fn(out, is_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(ptr), gdim, gstr, box,
-              estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 int tc_tile_n(int N) { return N <= 64 ? 64 : 128; }
-
-static bool g_use_2cta = false;   // measured on B200 (64x10 s): the pair kernel is not faster yet at M = 8064 (see DESIGN.md)
-void tc_set_2cta(bool on) { g_use_2cta = on; }
-void tc_set_debug(int bits) {
-    g_dbg = bits & 0xff;
-    const int mode = (bits >> 8) & 3;
-    cudaMemcpyToSymbol(g_store_mode, &mode, sizeof(int));
-    const int hint = (bits >> 10) & 3;
-    cudaMemcpyToSymbol(g_l2_hint_mode, &hint, sizeof(int));
-}
-void tc_print_timeline(int n_tiles) {   // after a 1-CTA launch with debug bit 5
-    long long h[64][8];
-    if (cudaMemcpyFromSymbol(h, g_timeline, sizeof(h)) != cudaSuccess) return;
-    const long long t0 = h[0][0];
-    for (int i = 0; i < n_tiles && i < 64; ++i)
-        fprintf(stderr, "    tile %2d: acc free %7lld  mma issued %7lld | acc full seen %7lld  stored %7lld   (epilogue %lld cyc: tmem %lld, maths %lld, 1st plane %lld)\n", i,
-                h[i][0] - t0, h[i][1] - t0, h[i][2] - t0, h[i][3] - t0, h[i][3] - h[i][2], h[i][4] - h[i][2], h[i][5] - h[i][4], h[i][6] - h[i][5]);
-}
-double tc_probe_mhz() {   // effective SM clock seen by CTA 0 of the last 1-CTA launch with a non-zero debug mask (bit 4 = probe only)
-    unsigned long long h[2] = {0, 0};
-    if (cudaMemcpyFromSymbol(h, g_clk_probe, sizeof(h)) != cudaSuccess || h[1] == 0) return 0.0;
-    return 1e3 * (double)h[0] / (double)h[1];
-}
 
 bool gemm_tc_cluster_supported(int N, int epi_kind, int cl) {
     return (cl == 2 || cl == 4) && N % (128 * cl) == 0 && (epi_kind == EPI_BIAS_SILU_ACT || epi_kind == EPI_GLU_F32 || epi_kind == EPI_QKV_ACT);
 }
 
-cudaError_t launch_gemm_tc(const TcOperand &A, const TcOperand &W, int M, int N, int K, bool split3,
-                           const EpiParams &epi, cudaStream_t st, int cl, const TcOperand *A_slice) {
+cudaError_t launch_gemm_tc(const TcOperand &A, const TcOperand &W, int M, int N, int K, bool split3, const EpiParams &epi, cudaStream_t st,
+                           int cl, const TcOperand *A_slice) {
     if (M <= 0 || N <= 0) return cudaSuccess;
     if (K % BK != 0 || A.box_rows != BM) return cudaErrorInvalidValue;
     if (split3 && !(A.has_lo && W.has_lo)) return cudaErrorInvalidValue;
@@ -972,10 +455,19 @@ cudaError_t launch_gemm_tc(const TcOperand &A, const TcOperand &W, int M, int N,
         default: return cl == 2 ? launch_kcl<3, EPI_QKV_ACT, 2>(*A_slice, W, M, N, K, epi, st) : launch_kcl<3, EPI_QKV_ACT, 4>(*A_slice, W, M, N, K, epi, st);
         }
     }
-    if (W.box_rows == 128 && N >= 256 && g_use_2cta)
-        return split3 ? launch_t2<3>(A, W, M, N, K, epi, st) : launch_t2<1>(A, W, M, N, K, epi, st);
     if (W.box_rows == 128) return split3 ? launch_t<128, 3>(A, W, M, N, K, epi, st) : launch_t<128, 1>(A, W, M, N, K, epi, st);
     if (W.box_rows == 64) return split3 ? launch_t<64, 3>(A, W, M, N, K, epi, st) : launch_t<64, 1>(A, W, M, N, K, epi, st);
+    return cudaErrorInvalidValue;
+}
+
+bool gemm_tc_ln_supported(int N) { return N == LN_CL * 128; }
+
+cudaError_t launch_gemm_tc_ln(const TcOperand &A, const TcOperand &W, int M, int N, int K, bool split3, const LnEpi &epi, cudaStream_t st) {
+    if (M <= 0) return cudaSuccess;
+    if (!gemm_tc_ln_supported(N) || K % BK != 0 || W.box_rows != 128 || !epi.ln1_w || !epi.ln1_b) return cudaErrorInvalidValue;
+    if (split3 && !(A.has_lo && W.has_lo)) return cudaErrorInvalidValue;
+    if (A.box_rows == BM / LN_CL) return split3 ? launch_ln<3, true>(A, W, M, N, K, epi, st) : launch_ln<1, true>(A, W, M, N, K, epi, st);
+    if (A.box_rows == BM) return split3 ? launch_ln<3, false>(A, W, M, N, K, epi, st) : launch_ln<1, false>(A, W, M, N, K, epi, st);
     return cudaErrorInvalidValue;
 }
 

@@ -1,4 +1,4 @@
-// kernels.h -- host-callable launchers of the sm_100a kernels (one .cu per op group).
+// kernels.h -- host-callable launchers of the sm_90a kernels (one .cu per op group).
 #pragma once
 #include <cuda.h>
 
@@ -75,7 +75,7 @@ void launch_subsample_dw(const float *in, const int32_t *in_rows, const int32_t 
 void launch_gemm_simt(const float *A, int lda, const float *W, int ldw, int M, int N, int K,
                       const EpiParams &epi, cudaStream_t st);
 
-// tcgen05 path (gemm_tc.cu): a K-major bf16 matrix [rows][K] as TMA tensor maps of its hi
+// wgmma path (gemm_tc.cu): a K-major bf16 matrix [rows][K] as TMA tensor maps of its hi
 // (and lo) split planes, box = 64 (K) x box_rows, SWIZZLE_128B.
 struct TcOperand {
     CUtensorMap hi, lo;
@@ -83,24 +83,19 @@ struct TcOperand {
     uint32_t box_rows = 0;
 };
 bool make_tc_operand(TcOperand *out, const bf16 *hi, const bf16 *lo, uint64_t rows, uint64_t K, uint32_t box_rows);
-// Output-side tensor map for the TMA-store epilogue: [rows][ld] matrix of bf16 (is_f32 = false: box 64 x 32) or fp32
-// (box 32 x 32), 128-byte inner box, SWIZZLE_128B.
-bool make_tc_out_map(CUtensorMap *out, const void *ptr, bool is_f32, uint64_t rows, uint64_t ld);
-int tc_tile_n(int N);
-void tc_set_2cta(bool on);   // debug/measurement switch: use the cta_group::2 kernel for N >= 256 (default off; PK_GEMM_2CTA=1)   // N-tile (= box_rows of the weight operand) chosen for an [N][K] weight
-void tc_set_debug(int bits); // measurement aid (PK_GEMM_DBG): bit 0 = skip the epilogue's work, bit 1 = skip the TMA loads (results are garbage)
-double tc_probe_mhz();
-void tc_print_timeline(int n_tiles);
+int tc_tile_n(int N);        // N-tile (= box_rows of the weight operand) chosen for an [N][K] weight
 // cl = 2 | 4 with A_slice = the A operand with a 128 / cl-row box: clusters of cl CTAs along N that share (TMA multicast) the
 // A tile; taken when gemm_tc_cluster_supported(N, epi.kind, cl), else the plain persistent kernel.
 bool gemm_tc_cluster_supported(int N, int epi_kind, int cl);
 cudaError_t launch_gemm_tc(const TcOperand &A, const TcOperand &W, int M, int N, int K, bool split3,
                            const EpiParams &epi, cudaStream_t st, int cl = 1, const TcOperand *A_slice = nullptr);
 
-// ------------------------------------------------------------------ gemm_tc_ln.cu (K5b: residual GEMM + fused LayerNorm)
+// Residual GEMM + fused LayerNorm (gemm_tc.cu, the same wgmma main loop):
 //     v = resid + alpha * (A . W^T + bias)   (resid may be null);   y1 = LN1(v);   y2 = LN2(y1) if ln2_w
 //     out_f32 = out_ln1 ? y1 : v   (may alias resid);   planes = hi/lo split of the last LayerNorm's result
-// N must be a full LayerNorm row of 4 x 128 columns (one 4-CTA cluster per 128-row block; statistics through DSMEM).
+// N must be a full LayerNorm row of 4 x 128 columns (one 4-CTA cluster per 128-row block; row statistics through
+// distributed shared memory).  A with a 32-row box (A.box_rows == 32): every CTA fetches a quarter of the A tile and
+// TMA-multicasts it to the cluster; with the 128-row box every CTA loads the whole tile.
 struct LnEpi {
     const float *bias = nullptr, *resid = nullptr;
     float alpha = 1.0f;
@@ -111,10 +106,7 @@ struct LnEpi {
     float eps = 1e-5f;
 };
 bool gemm_tc_ln_supported(int N);
-void gemm_tc_ln_set_debug(int on);            // measurement aid (PK_LN_DBG=1): per-tile epilogue timeline of CTA 0
-void gemm_tc_ln_print_timeline(int n_tiles);
-cudaError_t launch_gemm_tc_ln(const TcOperand &A, const TcOperand &W, int M, int N, int K, bool split3, const LnEpi &epi, int num_sms,
-                              cudaStream_t st);
+cudaError_t launch_gemm_tc_ln(const TcOperand &A, const TcOperand &W, int M, int N, int K, bool split3, const LnEpi &epi, cudaStream_t st);
 
 // ------------------------------------------------------------------ gemm_skinny.cu (M <= 128: the streaming path's GEMMs)
 size_t gemm_skinny_ws_floats(int max_n, int max_splits);
@@ -142,15 +134,12 @@ bool launch_relpos_attention_tc(const float *q32, const float *pos_u, const floa
                                 int ld_kv, const int32_t *row_off, int n_utt, int max_T, int n_heads, int head_dim, const bf16 *pp_hi,
                                 const bf16 *pp_lo, int tmax, int d_model, ActBuf out, cudaStream_t st);
 
-// tcgen05 variant (attention_umma.cu): head_dim 64, utterances of <= 128 frames, one CTA per (utterance, head).
-// kv = tensor maps of the [M][2 d] k | v planes (box 64 x 128, rows = M exactly); pp = of the [2 tmax - 1][d] planes of
-// the projected position table (box 64 x 256).
-bool relpos_attention_umma_supported(int head_dim, int max_T);
-bool launch_relpos_attention_umma(const float *q32, const float *pos_u, const float *pos_v, const TcOperand &kv, const TcOperand &pp,
-                                  const int32_t *row_off, int n_utt, int max_T, int n_heads, int head_dim, int tmax, int d_model, int num_sms, ActBuf out,
-                                  cudaStream_t st);
-void relpos_attention_umma_set_debug(int on);          // measurement aid (PK_AU_DBG=1): per-item timeline of CTA 0
-void relpos_attention_umma_print_timeline(int n_items);
+// wgmma variant (attention_wgmma.cu): head_dim 64, utterances of <= 128 frames, one CTA per (head, utterance); same
+// operands as launch_relpos_attention_tc.
+bool relpos_attention_wgmma_supported(int head_dim, int max_T);
+bool launch_relpos_attention_wgmma(const float *q32, const float *pos_u, const float *pos_v, const bf16 *kv_hi, const bf16 *kv_lo, int ld_kv,
+                                   const int32_t *row_off, int n_utt, int max_T, int n_heads, int head_dim, const bf16 *pp_hi, const bf16 *pp_lo,
+                                   int tmax, int d_model, ActBuf out, cudaStream_t st);
 
 // ContextTrie (src/phrase_boost.cpp:9-66) in CSR form on the device: node 0 = root; the edges of node i are
 // [first[i], first[i+1]) = (token, child node), sorted by token.

@@ -187,7 +187,7 @@ mel_logpower_kernel(const float *__restrict__ pcm, const int64_t *__restrict__ p
 }
 
 // K2: per-utterance, per-bin normalisation (audio.cpp:138-150: mean over the frames, UNBIASED variance, eps outside the root).
-// Round 1 ran it as one block per utterance (64 blocks on 148 SMs, three serial sweeps over the frames: 41 us).  Now every
+// One block per utterance would leave most SMs idle (64 blocks) and sweep the frames three times serially.  Instead every
 // utterance is cut into MEL_CH frame chunks: mel_stats_kernel reduces a chunk to (mean_c, M2_c = sum (x - mean_c)^2) per bin with
 // two sweeps over its own frames, mel_apply_kernel combines the MEL_CH partials of an utterance in a fixed order with Chan's
 // formula (mean = sum n_c mean_c / F, M2 = sum M2_c + n_c (mean_c - mean)^2: the accuracy of the two-pass form, deterministic,

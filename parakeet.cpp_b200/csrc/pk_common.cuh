@@ -1,4 +1,4 @@
-// pk_common.cuh -- shared declarations for the sm_100a kernels of the hot path.
+// pk_common.cuh -- shared declarations for the sm_90a kernels of the hot path.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -14,13 +14,10 @@ typedef __nv_bfloat16 bf16;
 // Every kernel of the path starts with pdl_wait() (griddepcontrol.wait: returns once the preceding grid has completed and
 // its writes are visible; a no-op for a normal launch) and is launched through launch_pdl(); with PK_PDL=1 the launch
 // carries programmatic stream serialisation, so the next grid's CTAs are scheduled and do their input-independent set-up
-// (barrier init, TMEM allocation, index math) while the previous grid drains.  Because EVERY kernel waits before its
+// (barrier init, index math) while the previous grid drains.  Because EVERY kernel waits before its
 // first global access, completion of a grid still implies completion of all its predecessors.
-// MEASURED (B200, profiles/r02_p_pdl.txt): with plain stream launches (PK_GRAPH=0) it helps (single-stream chunk 2.54 ->
-// 2.31 ms, 110m step 9.97 -> 9.90 ms); inside the CUDA graphs the product path replays it does not -- implicit trigger at
-// CTA exit: +-0.1 %; trigger at kernel entry: 2-8 % SLOWER (the early-resident CTAs of the next grid spin in
-// griddepcontrol.wait next to the running grid); trigger after the GEMM's last operand load: 1 % slower.  Graph edges
-// are already cheap, so the attribute is OFF by default (PK_PDL=1 turns it on).
+// The attribute is OFF by default (PK_PDL=1 turns it on): inside the CUDA graphs the product path replays, graph edges
+// are already cheap.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 #ifndef PK_PDL_TRIGGER
 #define PK_PDL_TRIGGER 1     // 0: implicit (at CTA exit); 1: at the top of every kernel; 2: only late in the GEMM (all loads issued)
@@ -79,7 +76,7 @@ struct PerDeviceFlag {
 };
 
 // An activation that feeds a GEMM as the A operand.  In PK_MATH_FP32 mode only
-// `f32` is set; in the tcgen05 modes the producer kernel writes the bf16 hi/lo
+// `f32` is set; in the tensor-core modes the producer kernel writes the bf16 hi/lo
 // split planes (hi = rn(x), lo = rn(x - hi)), which cost the same bytes as fp32.
 struct ActBuf {
     float *f32 = nullptr;
@@ -157,12 +154,6 @@ struct EpiParams {
     const float *resid = nullptr;
     float alpha = 1.0f;
     int qcols = 0;                // EPI_QKV_ACT: leading q columns (also the leading dimension of out_f32)
-    // tcgen05 kernels only: results leave the SM by TMA (cp.async.bulk.tensor shared -> global) instead of st.global.
-    // tm_out0 / tm_out1 are HOST pointers to CUtensorMaps of the output (fp32 matrix, or the bf16 hi / lo planes) with a
-    // 32-row x 128-byte box, SWIZZLE_128B (make_tc_out_map); the launcher copies them into kernel parameters.
-    // EPI_QKV_ACT: tm_out2 = the fp32 q matrix.
-    int tma_out = 0;
-    const void *tm_out0 = nullptr, *tm_out1 = nullptr, *tm_out2 = nullptr;
 };
 
 // Generic (edge-tile / run-time-kind) path; out of line so that it does not bloat the hot loops.
@@ -243,7 +234,7 @@ __device__ __forceinline__ float fast_sigmoid(float x) {
     return r;
 }
 
-// Split form used by the tcgen05 kernels: all global LOADS of a 16-column chunk (bias, residual)
+// Split form used by the tensor-core kernels: all global LOADS of a 16-column chunk (bias, residual)
 // are issued before the accumulator is read, then pure math, then all STORES -- otherwise every
 // epilogue4 call waits for its own L2 round trip (loads cannot be hoisted above the previous
 // call's stores: out_f32 may alias resid).

@@ -8,9 +8,9 @@
 //     CausalConformerConvModule::forward_cached            :41-80
 //   rnnt_streaming_decode_chunk                            src/eou.cpp:17-98
 //
-// B200 design: the reference advances ONE stream by 1-2 encoder frames per call, which is weight-bandwidth-bound (435 MB of
+// Design: the reference advances ONE stream by 1-2 encoder frames per call, which is weight-bandwidth-bound (435 MB of
 // fp32 weights per chunk).  Here S streams advance in LOCK STEP: a step takes one chunk of every stream, and all
-// streams' frames form one packed row block M = sum_s C_s that runs through the same tcgen05 GEMMs / LayerNorm kernels as
+// streams' frames form one packed row block M = sum_s C_s that runs through the same wgmma GEMMs / LayerNorm kernels as
 // the offline path (weights are read once per step for all streams).  Per-stream state is resident in HBM: sample
 // overlap + pre-emphasis carry, leftover mel frames, per layer a ring of the last att_context_left K / V rows and the
 // last k-1 GLU outputs, the LSTM state, the last token and the absolute frame offset.  All lengths depend only on the

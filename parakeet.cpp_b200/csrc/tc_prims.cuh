@@ -1,5 +1,5 @@
-// tc_prims.cuh -- the sm_100a primitives shared by the tcgen05 GEMM kernels (gemm_tc.cu, gemm_tc_ln.cu): mbarrier,
-// TMA loads, UMMA descriptors / issue / commit, TMEM loads, explicit shared-space accesses, cluster helpers.
+// tc_prims.cuh -- the sm_90a primitives of the wgmma GEMM kernels (gemm_tc.cu): mbarrier, TMA loads (plain and
+// multicast), thread-block cluster helpers, wgmma shared-memory descriptors, issue / commit / wait.
 #pragma once
 #include <cuda.h>
 
@@ -10,7 +10,7 @@ namespace tc {
 
 constexpr int BM = 128;
 constexpr int BK = 64;                 // 64 bf16 = 128 B = one SWIZZLE_128B row
-constexpr int UMMA_K = 16;
+constexpr int WGMMA_K = 16;
 
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -35,19 +35,20 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
         if (spin > (1u << 26)) __trap();   // ~seconds: protocol error, fail instead of hanging
     }
 }
-// L2 eviction-priority hints of the TMA operand loads (the 64-bit policy words CUTLASS uses for createpolicy-free hints).
-// Measured (profiles/r02_b_gemm_analysis.md): the result stream of a GEMM (66 MB per fc1 launch) pushes the operand tiles
-// that all CTAs re-read out of the near L2 partition -- lts hit rate 91 % -> 74 %, every miss a trip to the far die --
-// which is what stretched the MMA interval when loads and stores ran together.  Operands are therefore loaded EVICT_LAST.
-constexpr uint64_t L2_EVICT_NORMAL = 0x1000000000000000ull, L2_EVICT_FIRST = 0x12F0000000000000ull, L2_EVICT_LAST = 0x14F0000000000000ull;
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// L2 eviction-priority hint of the TMA operand loads (the 64-bit policy word CUTLASS uses for createpolicy-free hints):
+// every CTA re-reads the operand tiles, while the result stream of the GEMM would otherwise push them out of L2.
+constexpr uint64_t L2_EVICT_LAST = 0x14F0000000000000ull;
 __device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *tm, uint64_t *bar, int c0, int c1, uint64_t policy = L2_EVICT_LAST) {
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(policy)
         : "memory");
 }
-// The same load MULTICAST to the CTAs of `cta_mask` in this cluster: the tile lands at the same shared-memory offset in each of
-// them and completes its bytes on the mbarrier at the same offset in each of them (CUTLASS SM90_TMA_LOAD_MULTICAST_2D).
+// The same load MULTICAST to the CTAs of `cta_mask` in this cluster: the tile lands at the same shared-memory offset in each
+// of them and completes its bytes on the mbarrier at the same offset in each of them.
 __device__ __forceinline__ void tma_load_2d_mcast(void *smem_dst, const CUtensorMap *tm, uint64_t *bar, int c0, int c1, uint16_t cta_mask,
                                                   uint64_t policy = L2_EVICT_LAST) {
     asm volatile(
@@ -55,9 +56,29 @@ __device__ __forceinline__ void tma_load_2d_mcast(void *smem_dst, const CUtensor
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0), "r"(c1), "l"(policy)
         : "memory");
 }
-// One elected lane of a fully active warp (the warp-specialised roles below run under it): unlike `lane == 0`, ptxas
-// then knows that exactly one thread executes the region and issues UTCHMMA / UTMALDG from uniform registers directly
-// instead of wrapping every one of them in an ELECT / R2UR.BROADCAST / BRA.U.ANY serialisation loop.
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+// every thread of every CTA of the cluster; orders the shared::cluster accesses before it against those after it
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the address of the same shared-memory location in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_rank(uint32_t saddr, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
+    return r;
+}
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+}
+__device__ __forceinline__ void st_cluster_f32(uint32_t cluster_addr, float v) {
+    asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(cluster_addr), "f"(v) : "memory");
+}
+
+// One elected lane of a fully active warp: ptxas then knows that exactly one thread runs the region.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile(
@@ -67,105 +88,63 @@ __device__ __forceinline__ bool elect_one() {
         : "=r"(pred));
     return pred != 0;
 }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
 
-// K-major operand tile in shared memory, rows of 128 B, SWIZZLE_128B (as written by TMA):
-// 8-row core groups are 1024 B apart (SBO); LBO unused for swizzled K-major (1);
-// descriptor version 1 (Blackwell), layout type 2 = SWIZZLE_128B.  (cute mma_sm100_desc.hpp)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
+// K-major operand tile in shared memory, rows of 128 B, SWIZZLE_128B (as written by TMA), 1024-byte aligned:
+// 8-row core groups are 1024 B apart (SBO); LBO unused for swizzled K-major (1); layout type 1 = SWIZZLE_128B
+// (sm_90 GMMA descriptor: start >> 4 at [0,14), LBO >> 4 at [16,30), SBO >> 4 at [32,46), layout at [62,64)).
+// A K step of 16 bf16 inside the swizzle atom advances the start address by 32 B.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
     uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);          // start address  [0,14)
-    d |= (uint64_t)1 << 16;                           // leading byte offset (>>4) [16,30)
-    d |= (uint64_t)(1024 >> 4) << 32;                 // stride byte offset (>>4)  [32,46)
-    d |= (uint64_t)1 << 46;                           // version = 1               [46,48)
-    d |= (uint64_t)2 << 61;                           // SWIZZLE_128B              [61,64)
+    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// kind::f16 instruction descriptor: D=f32, A=B=bf16, both K-major, N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int m, int n) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D[64 x BN] (fp32, registers of the warpgroup) += A[64 x 16] . B[BN x 16]^T, both bf16 K-major in shared memory.
+// Thread t of the warpgroup holds rows 16 (t / 32) + (t % 32) / 4 (+ 8) and columns 8 j + 2 (t % 4) (+ 1): d[4 j .. 4 j + 3].
+template <int BN>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc);
+
+template <>
+__device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// arrives on `bar` (same offset) in every CTA of `cta_mask` once the MMAs issued so far have retired
-__device__ __forceinline__ void umma_commit_mcast(uint64_t *bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(cta_mask)
-                 : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns -> 16 registers per thread.  Issue only; the caller overlaps
-// the TMEM read latency with other work and calls tmem_wait_ld() before touching v[].
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t *v) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc));
 }
 
-// Explicit shared-space accesses for the epilogue staging (the compiler otherwise emits generic
-// LD/ST: the pointer is derived from a uintptr_t-aligned base).
-__device__ __forceinline__ void sts128(uint32_t a, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
-}
-__device__ __forceinline__ float4 lds128(uint32_t a) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
-    return v;
-}
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t *v) {
+template <>
+__device__ __forceinline__ void wgmma_bf16<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ uint4 lds128u(uint32_t a) {
-    uint4 v;
-    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a) : "memory");
-    return v;
-}
-__device__ __forceinline__ void split_pair(float x, float y, uint32_t &hi, uint32_t &lo) {
-    const __nv_bfloat162 h = __floats2bfloat162_rn(x, y);
-    const float2 hf = __bfloat1622float2(h);
-    const __nv_bfloat162 l = __floats2bfloat162_rn(x - hf.x, y - hf.y);
-    hi = *reinterpret_cast<const uint32_t *>(&h);
-    lo = *reinterpret_cast<const uint32_t *>(&l);
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t saddr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc));
 }
 
 }  // namespace tc

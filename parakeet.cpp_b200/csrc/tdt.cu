@@ -280,7 +280,7 @@ __device__ __forceinline__ void cluster_pass_n(const bf16 *W1, int RS1, int LO1,
 // Cheaper than cooperative_groups' grid.sync() and traps instead of hanging if a CTA never arrives.
 // (A hierarchical variant -- hardware cluster barrier, one atomic per cluster, second cluster barrier -- was measured
 // SLOWER: 5.4-6.1k cycles per use against 3.2-5.1k; two barrier.cluster round trips cost more than the 111 atomics saved.)
-// Same-address atomics serialise in the L2 (~27 cycles each: 148 of them made a barrier 3.2-5.1k cycles), so the arrivals
+// Same-address atomics serialise in the L2 (one arrival per CTA of the grid), so the arrivals
 // are spread over GBAR counters on different 128-byte lines (CTA c -> counter c % GBAR) and lanes 0..GBAR-1 of warp 0
 // poll one counter each.
 constexpr int GBAR = 8, GBAR_STRIDE = 32;      // counters, uints between them

@@ -267,7 +267,7 @@ def safetensors_probe(path: str, name: Optional[str] = None, cap: int = 0):
 
 
 def selftest_gemm(M, N, K, epi_kind, math=0, seed=1, device=0):
-    """-> (max_abs_err, max_abs_ref) of the tcgen05 GEMM vs the fp32 CUDA-core GEMM."""
+    """-> (max_abs_err, max_abs_ref) of the wgmma GEMM vs the fp32 CUDA-core GEMM."""
     L = load_library()
     e, r = C.c_float(), C.c_float()
     st = L.pk_selftest_gemm(device, M, N, K, epi_kind, math, seed, C.byref(e), C.byref(r))
@@ -277,7 +277,7 @@ def selftest_gemm(M, N, K, epi_kind, math=0, seed=1, device=0):
 
 
 def selftest_attention(lens, tmax=126, mode=0, seed=1, device=0):
-    """-> (max_abs_err, max_abs_ref) of the tcgen05 attention kernel vs the fp32 attention kernel."""
+    """-> (max_abs_err, max_abs_ref) of the wgmma attention kernel vs the fp32 attention kernel."""
     L = load_library()
     ln = np.ascontiguousarray(lens, np.int32)
     out = np.zeros(2, np.float32)
@@ -721,7 +721,7 @@ class Transcriber:
         else:
             opts = TranscribeOptions(decoder=decoder, timestamps=timestamps)
         if opts.boost_phrases:
-            raise NotImplementedError("phrase boosting is outside the B200 hot path (SURVEY.md section 8f.3)")
+            raise NotImplementedError("phrase boosting is outside the H100 hot path (SURVEY.md section 8f.3)")
         samples = read_wav(audio) if isinstance(audio, str) else np.asarray(audio, np.float32)
         dec = opts.decoder if self.config.has_ctc else Decoder.TDT
         toks = self.engine.transcribe_batch([samples], dec)[0]

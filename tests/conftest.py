@@ -1,5 +1,5 @@
 """pytest fixtures.  `-m "not gpu"` runs here (no GPU): oracle pinning, host logic, C-ABI
-exports.  `-m gpu` tests are the parity tests proper and call through the C-ABI on a B200."""
+exports.  `-m gpu` tests are the parity tests proper and call through the C-ABI on an H100."""
 from __future__ import annotations
 
 import os
@@ -16,7 +16,7 @@ import __graft_entry__ as ge  # noqa: E402
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def _has_gpu():
@@ -93,5 +93,9 @@ def m110(tmp_path_factory, pkg, O, synth):
 
 @pytest.fixture(scope="session")
 def golden():
-    p = os.path.join(ROOT, "tests", "golden", "golden_v1.npz")
-    return np.load(p, allow_pickle=False)
+    # one fixture set, stored in three files of < 1 MB each (tests/golden/make_golden.py)
+    g = {}
+    for name in ("golden_v1.npz", "golden_110m_v1.npz", "golden_110m_layers_v1.npz"):
+        with np.load(os.path.join(ROOT, "tests", "golden", name), allow_pickle=False) as f:
+            g.update({k: f[k] for k in f.files})
+    return g

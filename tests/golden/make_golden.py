@@ -91,9 +91,15 @@ def main():
     with tempfile.TemporaryDirectory() as td:
         run_model(out, "tiny", O.make_tiny_config(), 3, [(32000, 11), (20000, 12), (400, 13), (64000, 14)], td, True)
         run_model(out, "m110", O.make_110m_config(), 0, [(160000, 1000)], td, False)
-    path = os.path.join(ROOT, "tests", "golden", "golden_v1.npz")
-    np.savez_compressed(path, **out)
-    print("wrote", path, os.path.getsize(path) // 1024, "KiB")
+    # three files of < 1 MB each (tests/conftest.py merges them): tiny + decode vectors, 110m, 110m per-layer activations
+    big = lambda k: k.startswith("m110.") and (k.endswith("layers_first_last") or k.endswith(".sub"))
+    parts = {"golden_v1.npz": {k: v for k, v in out.items() if not k.startswith("m110.")},
+             "golden_110m_v1.npz": {k: v for k, v in out.items() if k.startswith("m110.") and not big(k)},
+             "golden_110m_layers_v1.npz": {k: v for k, v in out.items() if big(k)}}
+    for name, part in parts.items():
+        path = os.path.join(ROOT, "tests", "golden", name)
+        np.savez_compressed(path, **part)
+        print("wrote", path, os.path.getsize(path) // 1024, "KiB")
 
 
 def main_600m():
@@ -333,8 +339,67 @@ def main_boost():
     print("wrote", path, os.path.getsize(path) // 1024, "KiB")
 
 
+def main_live():
+    """What the tests that call the compiled reference directly compare against, for machines without it
+    (golden_live_v1.npz): parakeet::resample on the inputs of tests/test_abi.py and tests/test_gpu_parity.py, the
+    reference's mel / subsampling / per-layer encoder output / TDT decode of the tiny model, its chunk-by-chunk
+    streaming outputs and boosted CTC decodes (tests/test_oracle.py, live tests)."""
+    out = {}
+    rng = np.random.default_rng(4)
+    for i, (sr, dr, n) in enumerate([(44100, 16000, 9000), (48000, 16000, 5001), (8000, 16000, 2500), (22050, 16000, 3000), (24000, 16000, 999),
+                                     (96000, 16000, 6000), (16000, 16000, 50), (11025, 16000, 3), (16000, 8000, 1000), (44100, 16000, 0)]):
+        x = (rng.standard_normal(n) * 0.3).astype(np.float32)
+        if n > 0:
+            out[f"rs.cpu.{i}"] = R.resample(x, sr, dr)
+    rng = np.random.default_rng(9)
+    for i, (sr, dr, lens) in enumerate([(44100, 16000, [9000, 3, 20000]), (48000, 16000, [5001]), (8000, 16000, [2500, 1]), (22050, 16000, [30000, 12345]),
+                                        (96000, 16000, [6000]), (16000, 8000, [1000]), (11025, 16000, [4097])]):
+        for j, n in enumerate(lens):
+            x = (rng.standard_normal(n) * 0.3).astype(np.float32)
+            if n > 16:
+                out[f"rs.gpu.{i}.{j}"] = R.resample(x, sr, dr)
+    with tempfile.TemporaryDirectory() as td:
+        ocfg = O.make_tiny_config()
+        W = synth.make_weights(ocfg, seed=3)
+        wp, vp = os.path.join(td, "tiny_3.safetensors"), os.path.join(td, "tiny_3.vocab.txt")
+        synth.save_safetensors(wp, W)
+        synth.save_vocab(vp, synth.make_vocab(ocfg.vocab - 1, seed=3))
+        m = R.RefModel(wp, vp, 0, cfg=ocfg)
+        fr = R.mel(synth.make_audio(48000, 22))
+        sub_r, lay_r = m.encode_layers(fr, ocfg.d_model, ocfg.n_layers, O.encoder_len(fr.shape[0]))
+        out["tiny.mel"], out["tiny.sub"], out["tiny.layers"] = fr, sub_r, np.stack(lay_r)
+        out["tiny.tdt_tok"] = np.array([t[:3] for t in m.tdt_greedy(lay_r[-1], True)], np.int32).reshape(-1, 3)
+        m.close()
+        golden = np.load(os.path.join(ROOT, "tests", "golden", "golden_v1.npz"))
+        lp = O.ctc_log_probs(W, golden["tiny.c1.enc"])
+        rng = np.random.default_rng(23)
+        for k in range(5):
+            phrases = [rng.integers(0, ocfg.vocab - 1, size=int(rng.integers(1, 5))).tolist() for _ in range(8)]
+            out[f"boost.k{k}.ctc_tok"] = np.array([x[:3] for x in R.ctc_greedy_boosted(lp, ocfg.vocab - 1, phrases, 4.0)], np.int32).reshape(-1, 3)
+        socfg = O.make_tiny_stream_config()
+        Ws = synth.make_weights(socfg, seed=9)
+        wps = os.path.join(td, "ts9.safetensors")
+        synth.save_safetensors(wps, Ws)
+        sched = [2560, 3000, 800, 2560, 6000, 2560, 2560]
+        pcm = synth.make_audio(sum(sched), 91)
+        rs = R.RefStream(wps, socfg)
+        pos = 0
+        for ci, n in enumerate(sched):
+            rf, re_, rt = rs.chunk(pcm[pos:pos + n])
+            pos += n
+            out[f"stream.k{ci}.feats"] = np.zeros((0, socfg.mel_bins), np.float32) if rf is None else rf
+            out[f"stream.k{ci}.enc"] = np.zeros((0, socfg.d_model), np.float32) if re_ is None else re_
+            out[f"stream.k{ci}.tok"] = np.array([x[:3] for x in rt], np.int32).reshape(-1, 3)
+        rs.close()
+    path = os.path.join(ROOT, "tests", "golden", "golden_live_v1.npz")
+    np.savez_compressed(path, **out)
+    print("wrote", path, os.path.getsize(path) // 1024, "KiB")
+
+
 if __name__ == "__main__":
-    if len(sys.argv) > 1 and sys.argv[1] == "boost":
+    if len(sys.argv) > 1 and sys.argv[1] == "live":
+        main_live()
+    elif len(sys.argv) > 1 and sys.argv[1] == "boost":
         main_boost()
     elif len(sys.argv) > 1 and sys.argv[1] == "stream":
         main_stream()
