@@ -1085,7 +1085,15 @@ pk_status pk_selftest_gemm(int device, int M, int N, int K, int epi_kind, int ma
         if (rc == PK_OK && !use_skinny && getenv("PK_SELFTEST_TIME")) {   // warm, back-to-back timing of the wgmma launch
             cudaEvent_t e0, e1;
             cudaEventCreate(&e0); cudaEventCreate(&e1);
-            const int reps = 20;
+            // enough launches for a timed window of >= 50 ms (a shorter one measures clock ramp and scheduling), sized from
+            // 5 warm launches
+            float ms_probe = 0.f;
+            cudaEventRecord(e0, st);
+            for (int i = 0; i < 5; ++i) launch_gemm_tc(ta, tw, M, N, K, math == PK_MATH_BF16X3, ep, st, cl, &ta_sl);
+            cudaEventRecord(e1, st);
+            cudaStreamSynchronize(st);
+            cudaEventElapsedTime(&ms_probe, e0, e1);
+            const int reps = (int)std::min(20000.0, std::max(20.0, std::ceil(60.0 / std::max(ms_probe / 5.0, 1e-4))));
             cudaEventRecord(e0, st);
             for (int i = 0; i < reps; ++i) launch_gemm_tc(ta, tw, M, N, K, math == PK_MATH_BF16X3, ep, st, cl, &ta_sl);
             cudaEventRecord(e1, st);
@@ -1093,8 +1101,8 @@ pk_status pk_selftest_gemm(int device, int M, int N, int K, int epi_kind, int ma
             float ms = 0.f;
             cudaEventElapsedTime(&ms, e0, e1);
             const double us = 1e3 * ms / reps, tf = 2.0 * M * N * K / (us * 1e-6) / 1e12;
-            fprintf(stderr, "gemm_tc M=%d N=%d K=%d epi=%d math=%d: %.1f us  %.1f TFLOP/s algorithmic (x%d MMA)\n", M, N, K,
-                    epi_kind, math, us, tf, math == PK_MATH_BF16X3 ? 3 : 1);
+            fprintf(stderr, "gemm_tc M=%d N=%d K=%d epi=%d math=%d: %.2f us  %.1f TFLOP/s algorithmic (x%d MMA), %d launches in %.1f ms\n",
+                    M, N, K, epi_kind, math, us, tf, math == PK_MATH_BF16X3 ? 3 : 1, reps, ms);
             cudaEventDestroy(e0); cudaEventDestroy(e1);
         }
     }

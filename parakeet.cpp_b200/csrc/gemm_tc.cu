@@ -14,12 +14,17 @@
 // Structure (persistent, one CTA per SM, 384 threads = three warpgroups, static round-robin tile schedule, n-tile
 // fastest so that concurrently running CTAs share the same A rows through L2):
 //   warpgroup 0     TMA producer : one elected thread waits empty[s], arms full[s] with the byte count and issues the
-//                                  2 or 4 tile loads of k-block kb into stage s; it runs ahead across tiles, so the
-//                                  loads of tile i+1 overlap the epilogue of tile i
-//   warpgroups 1-2  consumers    : rows [64 (wg - 1), 64 wg) of the 128-row tile; per k-block wait full[s], 4 x (1|3)
-//                                  wgmma, commit; one wgmma group stays in flight and the stage of the previous
-//                                  k-block is released (empty[s], one arrival per consumer warp) once it has retired;
-//                                  then the epilogue straight from the accumulator registers
+//                                  2 or 4 tile loads of k-block kb into stage s; it runs ahead across tiles
+// The default kernel (gemm_tc_kernel) is PING-PONG: the producer hands most of its registers to the consumers
+// (setmaxnreg), and each consumer warpgroup owns whole 128 x BN tiles, the CTA's tiles alternating between the two:
+//   warpgroups 1-2  consumers    : wait for their turn (named barrier), then per k-block wait full[s], 4 x 2 x (1|3)
+//                                  wgmma (rows 0-63 and 64-127, same B operand), commit; one wgmma group stays in flight
+//                                  and the stage of the previous k-block is released (empty[s], one arrival per warp)
+//                                  once it has retired; after the last k-block is issued the other warpgroup's turn
+//                                  begins, and this one runs the epilogue from its registers under the other's wgmma
+// The cluster forms (gemm_tc_cl_kernel, gemm_tc_ln_kernel) keep the COOPERATIVE body (gemm_tc_body): both consumer
+// warpgroups work on one tile (rows [64 (wg - 1), 64 wg)) and run its epilogue together, which their cluster-wide
+// barriers need.
 // Every spin-wait is bounded and traps, so a protocol bug is an error, not a hung GPU.
 #include <cuda.h>
 
@@ -58,21 +63,33 @@ __device__ __forceinline__ void epilogue_regs(const float (&d)[BN / 2], const Ep
     const int q = lane & 3;
     const int row = row0 + (lane >> 2) + ((q & 1) ? 8 : 0);
     const bool vec_ok = ((epi.ldo & 3) == 0) && ((N & 3) == 0);
+    // The loads (bias, residual) of G column groups are issued before any of their stores: a load cannot be moved above
+    // an earlier store by the compiler (out_f32 may alias resid), so one group at a time would wait out one memory
+    // round trip per group.
+    constexpr int G = 4;
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-        // even lane: keeps its row-r pair, receives the partner's row-r pair; odd lane: the row-(r + 8) pairs
-        const float s0 = (q & 1) ? d[4 * j] : d[4 * j + 2], s1 = (q & 1) ? d[4 * j + 1] : d[4 * j + 3];
-        const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
-        if (row >= M) continue;
-        float4 v = (q & 1) ? make_float4(r0, r1, d[4 * j + 2], d[4 * j + 3]) : make_float4(d[4 * j], d[4 * j + 1], r0, r1);
-        const int col = n0 + 8 * j + 4 * (q >> 1);
-        if (vec_ok && col + 4 <= N) {
-            float4 b = make_float4(0.f, 0.f, 0.f, 0.f), r = b;
-            if (epi.bias) b = __ldg(reinterpret_cast<const float4 *>(epi.bias + col));
-            if (EK == EPI_RESID_F32) r = *reinterpret_cast<const float4 *>(epi.resid + (size_t)row * epi.ldo + col);
-            epi_store<EK>(epi, row, col, epi_math<EK>(v, b, r, epi.alpha));
-        } else {
-            epilogue4(epi_param, row, col, N, v);
+    for (int j0 = 0; j0 < BN / 8; j0 += G) {
+        float4 b[G], r[G];
+#pragma unroll
+        for (int g = 0; g < G; ++g) {
+            const int col = n0 + 8 * (j0 + g) + 4 * (q >> 1);
+            b[g] = r[g] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (row < M && vec_ok && col + 4 <= N) {
+                if (epi.bias) b[g] = __ldg(reinterpret_cast<const float4 *>(epi.bias + col));
+                if (EK == EPI_RESID_F32) r[g] = *reinterpret_cast<const float4 *>(epi.resid + (size_t)row * epi.ldo + col);
+            }
+        }
+#pragma unroll
+        for (int g = 0; g < G; ++g) {
+            const int j = j0 + g;
+            // even lane: keeps its row-r pair, receives the partner's row-r pair; odd lane: the row-(r + 8) pairs
+            const float s0 = (q & 1) ? d[4 * j] : d[4 * j + 2], s1 = (q & 1) ? d[4 * j + 1] : d[4 * j + 3];
+            const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+            if (row >= M) continue;
+            float4 v = (q & 1) ? make_float4(r0, r1, d[4 * j + 2], d[4 * j + 3]) : make_float4(d[4 * j], d[4 * j + 1], r0, r1);
+            const int col = n0 + 8 * j + 4 * (q >> 1);
+            if (vec_ok && col + 4 <= N) epi_store<EK>(epi, row, col, epi_math<EK>(v, b[g], r[g], epi.alpha));
+            else epilogue4(epi_param, row, col, N, v);
         }
     }
 }
@@ -159,7 +176,7 @@ __device__ __forceinline__ void epilogue_ln(const float (&d)[64], const LnEpi &e
     }
 }
 
-// The kernel body, shared by the three kernels below.
+// The cooperative kernel body of the cluster forms below.
 // CL > 1: thread-block clusters of CL CTAs along N.  The CL CTAs of a cluster work on the SAME 128-row block and on adjacent
 // column tiles, so the A tile of a k-block is the same for all of them.  MC: each CTA fetches 128 / CL of its rows (tmA_*
 // then have a 128 / CL-row box) and TMA-multicasts the slice into the stage of every CTA of the cluster; a stage is then
@@ -285,12 +302,120 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap &tmA_hi, const CU
     if (CL > 1) cluster_sync();      // nobody leaves while a peer may still multicast into it / arrive on its barriers
 }
 
+// The default GEMM, in the ping-pong form: each consumer warpgroup owns whole 128 x BN tiles (the CTA's units alternate
+// between them) and the two take turns in the mainloop, so one warpgroup's epilogue runs while the other issues wgmma.
+// Named barriers ORDER_BAR + cw say "warpgroup cw may start its next mainloop"; the other warpgroup arrives on it once it
+// has issued (not retired) the last wgmma of its own unit.  An arrival is made only if the waiting warpgroup has a unit
+// left, so no barrier is left half-arrived when the CTA exits.
+constexpr uint32_t ORDER_BAR = 1;
+constexpr uint32_t PRODUCER_REGS = 40, CONSUMER_REGS = 232;    // 128 x 40 + 256 x 232 <= 64 K registers of the SM
+
 template <int BN, int NPASS, int EK>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, int M, int N,
                int K, const __grid_constant__ EpiParams epi) {
-    gemm_tc_body<BN, NPASS, EK, 1, false, false>(tmA_hi, tmA_lo, tmW_hi, tmW_lo, M, N, K, epi, LnEpi());
+    using C = TcCfg<BN, NPASS>;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint64_t *full = reinterpret_cast<uint64_t *>(tiles + (size_t)C::STAGES * C::STAGE_BYTES), *empty = full + C::STAGES;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
+    const int nkb = K / BK;
+    const int tiles_n = (N + BN - 1) / BN, num_units = tiles_n * ((M + BM - 1) / BM);
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < C::STAGES; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], 4);       // the 4 warps of the warpgroup that consumed the stage
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    pdl_wait();      // barriers are set up while the previous grid drains; now its results are visible
+    pdl_trigger();
+
+    if (wg == 0) {
+        // ===================== TMA producer =====================
+        setmaxnreg_dec<PRODUCER_REGS>();
+        if (warp == 0 && elect_one()) {
+            uint32_t it = 0;   // global k-block counter across units
+            for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
+                const int m0 = (u / tiles_n) * BM, n0 = (u % tiles_n) * BN;
+                for (int kb = 0; kb < nkb; ++kb, ++it) {
+                    const int s = it % C::STAGES;
+                    const uint32_t ph = (it / C::STAGES) & 1;
+                    mbar_wait(&empty[s], ph ^ 1);
+                    uint8_t *st = tiles + (size_t)s * C::STAGE_BYTES;
+                    mbar_expect_tx(&full[s], C::STAGE_BYTES);
+                    tma_load_2d(st, &tmA_hi, &full[s], kb * BK, m0);
+                    if (NPASS == 3) tma_load_2d(st + C::A_BYTES + C::W_BYTES, &tmA_lo, &full[s], kb * BK, m0);
+                    tma_load_2d(st + C::A_BYTES, &tmW_hi, &full[s], kb * BK, n0);
+                    if (NPASS == 3) tma_load_2d(st + 2 * C::A_BYTES + C::W_BYTES, &tmW_lo, &full[s], kb * BK, n0);
+                }
+            }
+            pdl_trigger_late();     // every operand load of this CTA has been issued
+        }
+    } else {
+        // ===================== consumers: wgmma + epilogue, one whole tile each =====================
+        setmaxnreg_inc<CONSUMER_REGS>();
+        const int cw = wg - 1;       // this warpgroup takes units cw, cw + 2, cw + 4, ... of the CTA
+        auto release = [&](int s) {  // this warp has finished reading stage s
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[s]);
+        };
+        constexpr uint32_t HALF = 64u * 128u;    // rows 64..127 of the A tile: 64 rows of 128 B further on
+        uint32_t it = (uint32_t)(cw * nkb);      // the producer's k-block counter; the other warpgroup's units are skipped
+        for (int j = cw;; j += 2) {
+            const int u = (int)blockIdx.x + j * (int)gridDim.x;
+            if (u >= num_units) break;
+            const int m0 = (u / tiles_n) * BM, n0 = (u % tiles_n) * BN;
+            float d0[BN / 2], d1[BN / 2];        // rows 0..63 and 64..127 of the tile
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) d0[i] = d1[i] = 0.f;
+            fence_operands(d0);
+            fence_operands(d1);
+            if (j > 0) bar_sync(ORDER_BAR + cw, 256);     // the other warpgroup has issued its mainloop of unit j - 1
+            int prev_s = -1;
+            for (int kb = 0; kb < nkb; ++kb, ++it) {
+                const int s = it % C::STAGES;
+                const uint32_t ph = (it / C::STAGES) & 1;
+                mbar_wait(&full[s], ph);
+                const uint32_t st = smem_u32(tiles + (size_t)s * C::STAGE_BYTES);
+                const uint64_t a_hi = wgmma_desc_sw128(st), w_hi = wgmma_desc_sw128(st + C::A_BYTES);
+                const uint64_t a_lo = wgmma_desc_sw128(st + C::A_BYTES + C::W_BYTES);
+                const uint64_t w_lo = wgmma_desc_sw128(st + 2 * C::A_BYTES + C::W_BYTES);
+                const uint64_t a_hi1 = wgmma_desc_sw128(st + HALF), a_lo1 = wgmma_desc_sw128(st + C::A_BYTES + C::W_BYTES + HALF);
+                wgmma_fence();
+                // per accumulator the same MMA sequence as the cooperative body: k steps in order, hi.hi, hi.lo, lo.hi
+#pragma unroll
+                for (int k = 0; k < BK / WGMMA_K; ++k) {
+                    const uint64_t koff = (uint64_t)((k * WGMMA_K * 2) >> 4);   // 32 B per K step, encoded >> 4
+                    wgmma_bf16<BN>(d0, a_hi + koff, w_hi + koff);
+                    wgmma_bf16<BN>(d1, a_hi1 + koff, w_hi + koff);
+                    if (NPASS == 3) {
+                        wgmma_bf16<BN>(d0, a_hi + koff, w_lo + koff);
+                        wgmma_bf16<BN>(d1, a_hi1 + koff, w_lo + koff);
+                        wgmma_bf16<BN>(d0, a_lo + koff, w_hi + koff);
+                        wgmma_bf16<BN>(d1, a_lo1 + koff, w_hi + koff);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<1>();                            // the group of the previous k-block has retired
+                if (prev_s >= 0) release(prev_s);
+                prev_s = s;
+            }
+            it += (uint32_t)nkb;
+            if ((int)blockIdx.x + (j + 1) * (int)gridDim.x < num_units) bar_arrive(ORDER_BAR + (1 - cw), 256);
+            wgmma_wait<0>();
+            fence_operands(d0);
+            fence_operands(d1);
+            if (prev_s >= 0) release(prev_s);
+            const int lrow0 = (warp & 3) * 16;
+            epilogue_regs<BN, EK>(d0, epi, m0 + lrow0, n0, M, N, lane);
+            epilogue_regs<BN, EK>(d1, epi, m0 + 64 + lrow0, n0, M, N, lane);
+        }
+    }
 }
 
 // clusters of CL CTAs along N with the A tile multicast; 128-column tiles only

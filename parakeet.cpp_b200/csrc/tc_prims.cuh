@@ -101,6 +101,17 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
     d |= (uint64_t)1 << 62;
     return d;
 }
+// Named barriers 1..15 (0 is __syncthreads): bar_sync waits until `count` threads have arrived, bar_arrive only counts this one.
+__device__ __forceinline__ void bar_sync(uint32_t id, uint32_t count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+__device__ __forceinline__ void bar_arrive(uint32_t id, uint32_t count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+
+// Moves registers between the warpgroups of a CTA (every warp of the warpgroup executes it): the TMA producer gives up
+// most of its registers so that the consumer warpgroups can hold larger accumulators.
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
