@@ -50,6 +50,7 @@ struct PredictionConfig { int vocab_size = 1025, pred_hidden = 640, num_lstm_lay
 struct JointConfig { int encoder_hidden = 1024, pred_hidden = 640, joint_hidden = 640, vocab_size = 1025; };
 struct TDTConfig { EncoderConfig encoder; PredictionConfig prediction; JointConfig joint; std::vector<int> durations = {0, 1, 2, 3, 4}; };
 struct TDTCTCConfig { EncoderConfig encoder; PredictionConfig prediction; JointConfig joint; std::vector<int> durations = {0, 1, 2, 3, 4}; int ctc_vocab_size = 1025; };
+struct RNNTConfig { EncoderConfig encoder; PredictionConfig prediction; JointConfig joint; };   // config.hpp:47-53
 
 inline TDTCTCConfig make_110m_config() {       // config.hpp:77-95
     TDTCTCConfig c;
@@ -62,6 +63,9 @@ inline TDTConfig make_tdt_600m_config() {      // config.hpp:98-116
     c.encoder.mel_bins = 128;
     c.prediction.vocab_size = 8193; c.joint.vocab_size = 8193;
     return c;
+}
+inline RNNTConfig make_rnnt_600m_config() {     // config.hpp:118-135 (80 mels, vocab 1025)
+    return RNNTConfig{};
 }
 
 // ─── timestamps (timestamp.hpp:11-35) ────────────────────────────────────────
@@ -247,7 +251,10 @@ class EngineHolder {
     EngineHolder(const pk_config &cfg, const std::string &weights, int device) : cfg_(cfg) {
         if (pk_engine_create(&cfg, weights.c_str(), device, &e_) != PK_OK)
             throw std::runtime_error(std::string("parakeet_b200: ") + pk_last_error(nullptr));
-        cap_ = 2 * pk_encoder_frames(pk_mel_frames(cfg.max_samples)) + 8;
+        void *tok = nullptr;
+        int32_t row_ints = 0;
+        pk_token_buffer(e_, &tok, nullptr, &row_ints);
+        cap_ = row_ints - 1;     // the engine's token row capacity (2 T'max + 8; RNN-T: max_symbols T'max + 8)
     }
     EngineHolder(const EngineHolder &) = delete;
     EngineHolder &operator=(const EngineHolder &) = delete;
@@ -309,6 +316,8 @@ class TranscriberBase {
             pk_engine *e; bool on;
             ~BoostGuard() { if (on) pk_set_boost(e, nullptr, nullptr, 0, 0.f); }
         } guard{eng_->raw(), false};
+        if (!opts.boost_phrases.empty() && eng_->cfg().n_durations == 0)
+            throw std::runtime_error("RNNTTranscriber: phrase boosting covers CTC and TDT decodes only (phrase_boost.hpp)");
         if (!opts.boost_phrases.empty() && tokenizer_.loaded()) {
             ContextTrie trie;
             trie.build(opts.boost_phrases, tokenizer_);
@@ -410,6 +419,31 @@ class TDTTranscriber : public detail::TranscriberBase<TDTTranscriber> {
         return TranscriberBase::transcribe(samples, o);
     }
     pk_decoder pick(Decoder) const { return PK_DECODER_TDT; }
+};
+
+/// RNN-T models (ParakeetRNNT, reference src/rnnt.cpp; the CLI's --model rnnt-600m): TDTTranscriber's surface, decoded by
+/// rnnt_greedy_decode(_with_timestamps) (src/rnnt.cpp:56-177) on the device.  Non-empty boost_phrases throw.
+class RNNTTranscriber : public detail::TranscriberBase<RNNTTranscriber> {
+  public:
+    RNNTTranscriber(const std::string &weights_path, const std::string &vocab_path, const RNNTConfig &config = make_rnnt_600m_config(),
+                    int device = 0, int max_batch = 16, int max_samples = 30 * 16000, int max_symbols_per_step = 10) {
+        pk_config c;
+        pk_config_rnnt_600m(&c);
+        detail::fill(c, config.encoder, config.prediction, config.joint, {});
+        c.has_ctc = 0; c.joint_prefix_tdt = 0; c.max_symbols = max_symbols_per_step; c.max_batch = max_batch; c.max_samples = max_samples;
+        eng_ = std::make_unique<detail::EngineHolder>(c, weights_path, device);
+        tokenizer_.load(vocab_path);
+    }
+    using TranscriberBase::transcribe;
+    TranscribeResult transcribe(const std::string &audio_path, bool timestamps = false) {
+        TranscribeOptions o; o.timestamps = timestamps;
+        return TranscriberBase::transcribe(audio_path, o);
+    }
+    TranscribeResult transcribe(const std::vector<float> &samples, bool timestamps = false) {
+        TranscribeOptions o; o.timestamps = timestamps;
+        return TranscriberBase::transcribe(samples, o);
+    }
+    pk_decoder pick(Decoder) const { return PK_DECODER_RNNT; }
 };
 
 

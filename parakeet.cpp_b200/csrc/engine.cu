@@ -277,7 +277,10 @@ pk_status pk_engine::load(const char *path) {
     const std::string jp = c.joint_prefix_tdt ? "tdt_joint_." : "joint_.";
     if ((s = make_weight(st, jp + "enc_proj_.weight", jp + "enc_proj_.bias", J, d, enc_proj))) return s;
     if ((s = get_vec(st, jp + "pred_proj_.weight", J * P, &Wp))) return s;
-    {
+    if (D == 0) {   // RNNTJoint (rnnt.cpp:30-44): one output head out_proj_ over the V labels
+        if ((s = get_vec(st, jp + "out_proj_.weight", V * J, &Wout))) return s;
+        if ((s = get_vec(st, jp + "out_proj_.bias", V, &bout))) return s;
+    } else {
         std::vector<float> w((size_t)(V + D) * J), b((size_t)V + D), t;
         if (!st.read_f32(jp + "label_proj_.weight", t, (int64_t)V * J, e)) return fail(PK_ERR_MISSING, e);
         memcpy(w.data(), t.data(), t.size() * 4);
@@ -736,7 +739,7 @@ pk_status pk_engine::run_tdt() {
     const int bp = ((n_utt + 31) / 32) * 32;
     TdtParams p{};
     p.P = c.pred_hidden; p.J = c.joint_hidden; p.V = c.vocab; p.D = c.n_durations; p.L = c.lstm_layers;
-    p.Bpad = bp; p.n_utt = n_utt; p.cap = cap; p.n_dur = c.n_durations;
+    p.Bpad = bp; p.n_utt = n_utt; p.cap = cap; p.n_dur = c.n_durations; p.max_sym = c.max_symbols;
     p.max_steps = maxT + cap + 2;
     for (int i = 0; i < 8; ++i) p.durations[i] = c.durations[i];
     p.EP = EP; p.row_off = d_row_off; p.G0 = G0;
@@ -860,6 +863,14 @@ void pk_config_tdt_600m(pk_config *c) {
     c->has_ctc = 0; c->joint_prefix_tdt = 0; c->max_batch = 16; c->max_samples = 480000;
 }
 
+void pk_config_rnnt_600m(pk_config *c) {
+    pk_config_110m(c);
+    c->d_model = 1024; c->n_layers = 24; c->ff = 4096; c->lstm_layers = 2;
+    c->n_durations = 0;
+    for (int i = 0; i < 8; ++i) c->durations[i] = 0;
+    c->has_ctc = 0; c->joint_prefix_tdt = 0; c->max_symbols = 10; c->max_batch = 16; c->max_samples = 480000;
+}
+
 int32_t pk_mel_frames(int64_t n_samples) { return (int32_t)(1 + n_samples / 160); }
 int32_t pk_encoder_frames(int32_t f) { return conv_len(conv_len(conv_len(f))); }
 
@@ -882,9 +893,19 @@ pk_status pk_engine_create(const pk_config *cfg, const char *path, int device, p
     const pk_config &c = *cfg;
     if (c.d_model % 128 || c.d_model % c.n_heads || c.mel_bins % 8 || c.sub_channels % 4 || c.ff % 16 ||
         c.pred_hidden % 32 || c.joint_hidden % 32 || c.lstm_layers < 1 || c.lstm_layers > PK_MAX_LSTM ||
-        c.n_durations < 1 || c.n_durations > 8 || c.max_batch < 1 || c.max_samples < 400 || c.sub_channels > 1024) {
+        c.n_durations < 0 || c.n_durations > 8 || c.max_batch < 1 || c.max_samples < 400 || c.sub_channels > 1024) {
         g_create_err = "unsupported model shape in pk_config";
         return PK_ERR_INVALID;
+    }
+    if (c.n_durations == 0) {      // RNN-T joint (ParakeetRNNT, rnnt.cpp:48-52)
+        if (c.joint_prefix_tdt != 0 || c.has_ctc != 0) {
+            g_create_err = "RNN-T model (n_durations = 0): ParakeetRNNT has keys \"joint_.\" (joint_prefix_tdt = 0) and no CTC head (has_ctc = 0)";
+            return PK_ERR_INVALID;
+        }
+        if (c.max_symbols < 1 || c.max_symbols > 64) {
+            g_create_err = "RNN-T model (n_durations = 0): max_symbols must be in 1..64";
+            return PK_ERR_INVALID;
+        }
     }
     if (c.math != PK_MATH_FP32 && c.math != PK_MATH_BF16X3 && c.math != PK_MATH_BF16X1) {
         g_create_err = "unknown pk_math mode";
@@ -930,7 +951,8 @@ pk_status pk_engine_create(const pk_config *cfg, const char *path, int device, p
     e->f1n = conv_len(c.mel_bins);
     e->f2n = conv_len(e->f1n);
     e->f3n = conv_len(e->f2n);
-    e->cap = 2 * e->Tmax + 8;
+    // token row capacity: RNN-T emits at most max_symbols tokens per frame, so its hypotheses are never cut
+    e->cap = (c.n_durations == 0 ? c.max_symbols : 2) * e->Tmax + 8;
     pk_status s = e->load(path);
     if (s == PK_OK) s = e->alloc_workspace();
     if (s != PK_OK) {
@@ -1494,6 +1516,16 @@ static pk_status run_front(pk_engine *e) {
     e->front_done = true;
     return PK_OK;
 }
+// TDT and RNN-T share the decode kernel but not the joint: each decoder runs only on its own model
+// (a model without a CTC head rejects PK_DECODER_CTC in run_ctc).
+static pk_status check_decoder(pk_engine *e, pk_decoder dec) {
+    const bool rnnt_model = e->cfg.n_durations == 0;
+    if (dec == PK_DECODER_TDT && rnnt_model)
+        return e->fail(PK_ERR_INVALID, "PK_DECODER_TDT on an RNN-T model (n_durations = 0): use PK_DECODER_RNNT");
+    if (dec == PK_DECODER_RNNT && !rnnt_model)
+        return e->fail(PK_ERR_INVALID, "PK_DECODER_RNNT on a TDT model: use PK_DECODER_TDT");
+    return PK_OK;
+}
 static pk_status run_pipeline(pk_engine *e, pk_decoder dec) {   // everything after the front end
     pk_status s;
     if ((s = e->run_encoder(nullptr, nullptr))) return s;
@@ -1506,12 +1538,13 @@ pk_status pk_run_staged(pk_engine *e, pk_decoder dec) {
     if (!e || e->n_utt <= 0) return PK_ERR_INVALID;
     cudaSetDevice(e->device);
     if (e->gemm_err) return e->gemm_err;
+    if (pk_status ds = check_decoder(e, dec)) return ds;
     {
         pk_status fs = run_front(e);
         e->front_done = false;      // a second pk_run_staged of the same staged batch re-runs the front end
         if (fs) return fs;
     }
-    std::string key(1, dec == PK_DECODER_CTC ? 'c' : 't');
+    std::string key(1, dec == PK_DECODER_CTC ? 'c' : (dec == PK_DECODER_RNNT ? 'r' : 't'));
     const int32_t bg = e->boost_on ? e->boost_gen : 0;
     key.append(reinterpret_cast<const char *>(&bg), sizeof(bg));
     key.append(reinterpret_cast<const char *>(e->frame_off.data()), e->frame_off.size() * sizeof(int32_t));
@@ -1774,6 +1807,8 @@ pk_status pk_resample_batch(pk_engine *e, const float *pcm, const int64_t *offse
 // sorted by token) and uploaded; the decode kernels (ctc.cu: ctc_boosted_decode_kernel, tdt.cu: boost_on) walk it.
 pk_status pk_set_boost(pk_engine *e, const int32_t *phrase_ids, const int32_t *phrase_off, int32_t n_phrases, float boost) {
     if (!e || n_phrases < 0 || (n_phrases > 0 && (!phrase_ids || !phrase_off))) return PK_ERR_INVALID;
+    if (e->cfg.n_durations == 0 && n_phrases > 0)
+        return e->fail(PK_ERR_INVALID, "pk_set_boost: phrase boosting covers CTC and TDT decodes; this is an RNN-T model");
     cudaSetDevice(e->device);
     cudaStreamSynchronize(e->stream);
     ++e->boost_gen;
@@ -1911,6 +1946,7 @@ pk_status pk_decode(pk_engine *e, const float *enc, const int32_t *enc_lens, int
     if (!e || !enc || !enc_lens) return PK_ERR_INVALID;
     cudaSetDevice(e->device);
     pk_status s;
+    if ((s = check_decoder(e, dec))) return s;
     if ((s = stage_enc(e, enc, enc_lens, n_utt))) return s;
     if ((s = (dec == PK_DECODER_CTC ? e->run_ctc(nullptr) : e->run_tdt()))) return s;
     return e->fetch(out);

@@ -160,6 +160,7 @@ void launch_ctc_collapse(const int32_t *best, const float *conf, const int32_t *
 // ------------------------------------------------------------------ tdt.cu (K10)
 struct TdtParams {
     int P, J, V, D, L, Bpad, n_utt, cap, max_steps, n_dur;
+    int max_sym;                                      // RNN-T (n_dur == 0): max_symbols_per_step; unused by TDT
     int out_in_smem, wih_in_smem, smem_lstm_floats;   // filled by launch_tdt_decode
     int wstage_rows;                                  // rows of the shared-memory staging tile for weights that stay in L2 (0: none)
     int durations[8];

@@ -41,7 +41,7 @@ class _PkTokens(C.Structure):
                 ("end", C.POINTER(C.c_int32)), ("conf", C.POINTER(C.c_float)), ("len", C.POINTER(C.c_int32))]
 
 
-EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_engine_create", "pk_engine_destroy", "pk_last_error",
+EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_engine_create", "pk_engine_destroy", "pk_last_error",
            "pk_mel_frames", "pk_encoder_frames", "pk_mel", "pk_encode", "pk_decode", "pk_ctc_logprobs",
            "pk_transcribe_batch", "pk_stage_pcm", "pk_prefetch_pcm", "pk_run_staged", "pk_fetch_tokens", "pk_sync",
            "pk_token_buffer", "pk_stream", "pk_launch_count", "pk_profile_begin", "pk_profile_end",
@@ -69,6 +69,7 @@ def load_library():
     vp, i32p, f32p, i64p = C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_float), C.POINTER(C.c_int64)
     L.pk_config_110m.argtypes = [C.POINTER(_PkConfig)]
     L.pk_config_tdt_600m.argtypes = [C.POINTER(_PkConfig)]
+    L.pk_config_rnnt_600m.argtypes = [C.POINTER(_PkConfig)]
     L.pk_engine_create.argtypes = [C.POINTER(_PkConfig), C.c_char_p, C.c_int, C.POINTER(vp)]
     L.pk_engine_destroy.argtypes = [vp]
     L.pk_last_error.argtypes = [vp]
@@ -156,9 +157,10 @@ class ModelConfig:
     pred_hidden: int = 640
     lstm_layers: int = 1
     joint_hidden: int = 640
-    durations: tuple = (0, 1, 2, 3, 4)
+    durations: tuple = (0, 1, 2, 3, 4)    # () = RNN-T joint (ParakeetRNNT: out_proj_, no duration head)
     has_ctc: bool = True
     joint_prefix: str = "tdt_joint_."
+    max_symbols: int = 10                 # max_symbols_per_step (RNN-T: forced advance after this many)
     name: str = "tdt-ctc-110m"
     # streaming encoder only (StreamingEncoderConfig, streaming_encoder.hpp:18-24)
     att_context_left: int = 70
@@ -178,9 +180,13 @@ class ModelConfig:
             c.durations[i] = d
         c.has_ctc = int(self.has_ctc)
         c.joint_prefix_tdt = int(self.joint_prefix == "tdt_joint_.")
-        c.max_symbols = 10
+        c.max_symbols = self.max_symbols
         c.max_batch, c.max_samples, c.math = self.max_batch, self.max_samples, int(self.math)
         return c
+
+    @property
+    def is_rnnt(self) -> bool:
+        return len(self.durations) == 0
 
 
 def make_110m_config(**kw) -> ModelConfig:           # config.hpp:77-95
@@ -190,6 +196,13 @@ def make_110m_config(**kw) -> ModelConfig:           # config.hpp:77-95
 def make_tdt_600m_config(**kw) -> ModelConfig:       # config.hpp:98-116
     base = dict(mel_bins=128, d_model=1024, n_layers=24, ff=4096, vocab=8193, lstm_layers=2, has_ctc=False,
                 joint_prefix="joint_.", name="tdt-600m", max_batch=16, max_samples=480000)
+    base.update(kw)
+    return ModelConfig(**base)
+
+
+def make_rnnt_600m_config(**kw) -> ModelConfig:      # config.hpp:118-135 (ParakeetRNNT registers "joint_", rnnt.cpp:48-52)
+    base = dict(d_model=1024, n_layers=24, ff=4096, vocab=1025, lstm_layers=2, durations=(), has_ctc=False,
+                joint_prefix="joint_.", name="rnnt-600m", max_batch=16, max_samples=480000)
     base.update(kw)
     return ModelConfig(**base)
 
@@ -218,10 +231,20 @@ def make_tiny_config(**kw) -> ModelConfig:
     return ModelConfig(**base)
 
 
+def make_tiny_rnnt_config(**kw) -> ModelConfig:
+    """Small test-only RNN-T shape (not a reference preset)."""
+    base = dict(sub_channels=64, d_model=128, n_layers=2, n_heads=2, ff=256, vocab=33, pred_hidden=64,
+                joint_hidden=64, durations=(), has_ctc=False, joint_prefix="joint_.", name="tiny-rnnt",
+                max_batch=8, max_samples=64000)
+    base.update(kw)
+    return ModelConfig(**base)
+
+
 # ------------------------------------------------------------------ result types (timestamp.hpp, transcribe.hpp)
 class Decoder(enum.IntEnum):          # transcribe.hpp:34
     CTC = 0
     TDT = 1
+    RNNT = 2
 
 
 @dataclass
@@ -360,7 +383,7 @@ class Engine:
         if st != 0:
             raise RuntimeError(f"pk_engine_create failed ({st}): " + self.L.pk_last_error(None).decode())
         self.Tmax = self.L.pk_encoder_frames(self.L.pk_mel_frames(cfg.max_samples))
-        self.cap = 2 * self.Tmax + 8
+        self.cap = self.token_buffer()[2] - 1       # the engine's token row capacity (2 T'max + 8; RNN-T: max_symbols T'max + 8)
 
     def close(self):
         if self.h:
@@ -715,6 +738,12 @@ class Transcriber:
                 r.word_timestamps = self.tokenizer.group_words(toks)
         return r
 
+    def _decoder(self, decoder):
+        """An RNN-T model always decodes with RNNT; a model without a CTC head always with TDT."""
+        if self.config.is_rnnt:
+            return Decoder.RNNT
+        return decoder if self.config.has_ctc else Decoder.TDT
+
     def transcribe(self, audio, decoder=Decoder.TDT, timestamps: bool = False) -> TranscribeResult:
         if isinstance(decoder, TranscribeOptions):
             opts = decoder
@@ -723,8 +752,7 @@ class Transcriber:
         if opts.boost_phrases:
             raise NotImplementedError("phrase boosting is outside the H100 hot path (SURVEY.md section 8f.3)")
         samples = read_wav(audio) if isinstance(audio, str) else np.asarray(audio, np.float32)
-        dec = opts.decoder if self.config.has_ctc else Decoder.TDT
-        toks = self.engine.transcribe_batch([samples], dec)[0]
+        toks = self.engine.transcribe_batch([samples], self._decoder(opts.decoder))[0]
         return self._result(toks, opts.timestamps)
 
     def transcribe_batch(self, audios, decoder=Decoder.TDT, timestamps: bool = False) -> List[TranscribeResult]:
@@ -732,9 +760,10 @@ class Transcriber:
         out = []
         B = self.config.max_batch
         for i in range(0, len(pcms), B):
-            for toks in self.engine.transcribe_batch(pcms[i:i + B], decoder):
+            for toks in self.engine.transcribe_batch(pcms[i:i + B], self._decoder(decoder)):
                 out.append(self._result(toks, timestamps))
         return out
 
 
 TDTTranscriber = Transcriber   # transcribe.hpp:200-299 (same surface, TDT only)
+RNNTTranscriber = Transcriber  # same surface; an RNN-T config (make_rnnt_600m_config) decodes with Decoder.RNNT
