@@ -261,6 +261,38 @@ pk_status pk_selftest_gemm_ln(int device, int M, int K, int mode, int math, uint
  * zero position table; bit 1: zero keys.  err2 = {max |ctx - ctx_ref|, max |ctx_ref|}. */
 pk_status pk_selftest_attention(int device, const int32_t *lens, int n, int tmax, int mode, uint32_t seed, float *err2);
 
+/* Kernel test hooks (csrc/kernel_hooks.cu): each runs ONE launcher of the hot path exactly as the engine calls it, on host fp32
+ * arrays, on a private stream, synchronously, and returns every output buffer whole (bf16 planes widened to float).  Every
+ * device output sits between 64 KiB guard bands; output and guards start as 0xFF bytes (NaN in fp32 and bf16), so elements
+ * the kernel must not write come back NaN, and *guard_bad = the number of guard bytes that changed.
+ *
+ * GEMM: path 0 = fp32 CUDA-core kernel (math PK_MATH_FP32), 1 = wgmma (cluster 2 | 4: the multicast form, where
+ * supported), 2 = the few-row kernel (M <= 128, launched twice).  A [M][K], W [N][K], bias [N] (or NULL).  Output [M][ldo]:
+ * out_f32 for the fp32 kinds and GLU (N/2 columns), out_hi (| out_lo, NULL = no lo plane) for the act kinds and the k | v
+ * part of EPI_QKV_ACT (whose q columns go to out_f32 [M][qcols]); the act kinds write out_f32 on path 0.  EPI_RESID_F32
+ * reads resid [M][ldo]; in_place = 1 starts out_f32 as resid and passes it as both, as the encoder runs it. */
+pk_status pk_kernel_gemm(int device, int path, int math, int cluster, int M, int N, int K, int epi_kind, int qcols, int ldo, float alpha,
+                         int in_place, const float *A, const float *W, const float *bias, const float *resid, float *out_f32,
+                         float *out_hi, float *out_lo, int64_t *guard_bad);
+/* Relative-position attention: kernel 0 = fp32 CUDA-core, 1 = mma.sync (default), 2 = wgmma.  qkv [rows_total][3 d] (kernels 1
+ * and 2 get q in fp32 and k | v as bf16 planes, as the EPI_QKV_ACT epilogue lays them out), pp [2 tmax - 1][d], utterance
+ * b = rows [row_off[b], row_off[b+1]) (rows outside every utterance may exist).  ctx [rows_total][d]: ctx_f32 with
+ * PK_MATH_FP32 (kernel 0 only), else ctx_hi and, with PK_MATH_BF16X3, ctx_lo. */
+pk_status pk_kernel_attention(int device, int kernel, int math, int n_utt, const int32_t *row_off, int rows_total, int d_model, int n_heads,
+                              int tmax, const float *qkv, const float *pp, const float *pos_u, const float *pos_v, float *ctx_f32,
+                              float *ctx_hi, float *ctx_lo, int64_t *guard_bad);
+/* LayerNorm of x [M][d] (w2 == NULL: one; else LN2(LN1(x)), the chained form).  want_f32: y1 = LN1(x) written in place over
+ * x -> y1_f32.  planes (the operand of the last LayerNorm): 0 none, 1 hi, 2 hi + lo, 3 fp32 -> act_f32. */
+pk_status pk_kernel_layernorm(int device, int M, int d, const float *x, const float *w1, const float *b1, const float *w2, const float *b2,
+                              int want_f32, int planes, float *y1_f32, float *act_f32, float *hi, float *lo, int64_t *guard_bad);
+/* Depthwise conv (ks taps, tap-major w [ks][d], folded BatchNorm bias [d]) + SiLU over packed utterances of g [rows_total][d].
+ * Output [rows_total][d]: out_f32 with PK_MATH_FP32, else hi and, with PK_MATH_BF16X3, lo. */
+pk_status pk_kernel_dwconv(int device, int math, int n_utt, const int32_t *row_off, int rows_total, int d, int ks, const float *g,
+                           const float *w_tapmajor, const float *bias, float *out_f32, float *hi, float *lo, int64_t *guard_bad);
+/* CTC head reduction of logits [M][ld]: best [M] (first maximum), conf [M] = exp(max log-prob), logprobs [M][V] (or NULL). */
+pk_status pk_kernel_ctc_argmax(int device, int M, int V, int ld, const float *logits, int32_t *best, float *conf, float *logprobs,
+                               int64_t *guard_bad);
+
 /* Host-side text helpers (pure C++ host code; no device work):
  * Tokenizer::load/decode (src/vocab.cpp:10-64), group_timestamps (src/timestamp.cpp:24-75). */
 typedef struct pk_vocab pk_vocab;

@@ -45,7 +45,8 @@ ctc_frame_argmax_kernel(const float *__restrict__ logits, int M, int V, int ld, 
     for (int v = lane; v < V; v += 32) s += expf(l[v] - mx);
     s = warp_sum(s);
     if (lane == 0) {
-        best[row] = idx;
+        // no element > -inf (all -inf or NaN): the reference's scan starts at index 0 and keeps it
+        best[row] = idx == 0x7fffffff ? 0 : idx;
         conf[row] = 1.0f / s;
     }
     if (logprobs) {

@@ -1,0 +1,327 @@
+// kernel_hooks.cu -- pk_kernel_*: run ONE launcher of the hot path exactly as the engine calls it, on caller-supplied host
+// fp32 arrays, and hand back every output buffer whole (tests/test_kernels_fp64.py checks them against float64 math).
+//
+// Every device output buffer sits between two guard bands of kGuard bytes, and guards and output are pre-filled with 0xFF
+// bytes (NaN in fp32 and in bf16).  Each hook returns the number of guard bytes that changed in *guard_bad; elements the
+// kernel must not write come back still holding the pattern, so the caller can check the exact set of written elements.
+// bf16 planes come back widened to fp32 (exact).  A private stream, synchronous; nothing is cached between calls.
+#include <algorithm>
+#include <cstring>
+#include <vector>
+
+#include "../../include/parakeet_b200.h"
+#include "kernels.h"
+
+using namespace pk;
+
+namespace {
+
+constexpr size_t kGuard = (size_t)64 << 10;
+
+// Device buffers of one hook call; freed (and the stream destroyed) on scope exit.
+struct HookCtx {
+    cudaStream_t st = nullptr;
+    std::vector<void *> ptrs;
+    struct Guarded {
+        uint8_t *base;
+        size_t bytes;
+    };
+    std::vector<Guarded> outs;
+    bool ok = true;
+
+    explicit HookCtx(int device) {
+        ok = cudaSetDevice(device) == cudaSuccess && cudaStreamCreate(&st) == cudaSuccess;   // blocking: ordered after the memsets and copies
+    }
+    ~HookCtx() {
+        if (st) cudaStreamSynchronize(st);
+        for (void *p : ptrs) cudaFree(p);
+        if (st) cudaStreamDestroy(st);
+    }
+    void *alloc(size_t bytes) {
+        void *p = nullptr;
+        if (cudaMalloc(&p, bytes < 16 ? 16 : bytes) != cudaSuccess) {
+            ok = false;
+            return nullptr;
+        }
+        ptrs.push_back(p);
+        return p;
+    }
+    template <typename T>
+    T *upload(const T *h, size_t n) {
+        T *d = static_cast<T *>(alloc(n * sizeof(T)));
+        if (d && h && n && cudaMemcpy(d, h, n * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) ok = false;
+        return d;
+    }
+    // output buffer of `bytes` inside [guard | bytes | guard], all 0xFF
+    template <typename T>
+    T *guarded(size_t n) {
+        const size_t bytes = n * sizeof(T);
+        uint8_t *b = static_cast<uint8_t *>(alloc(bytes + 2 * kGuard));
+        if (!b) return nullptr;
+        if (cudaMemset(b, 0xFF, bytes + 2 * kGuard) != cudaSuccess) ok = false;
+        outs.push_back({b, bytes});
+        return reinterpret_cast<T *>(b + kGuard);
+    }
+    bool sync() { return ok && cudaStreamSynchronize(st) == cudaSuccess && cudaGetLastError() == cudaSuccess; }
+    int64_t guard_bad() {
+        int64_t bad = 0;
+        std::vector<uint8_t> h(kGuard);
+        for (const Guarded &g : outs)
+            for (const uint8_t *p : {g.base, g.base + kGuard + g.bytes}) {
+                if (cudaMemcpy(h.data(), p, kGuard, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+                for (uint8_t v : h) bad += v != 0xFF;
+            }
+        return bad;
+    }
+    pk_status finish(int64_t *guard_bad_out) {
+        if (!sync()) return PK_ERR_CUDA;
+        const int64_t gb = guard_bad();
+        if (gb < 0) return PK_ERR_CUDA;
+        if (guard_bad_out) *guard_bad_out = gb;
+        return PK_OK;
+    }
+};
+
+bool fetch_f32(float *host, const float *dev, size_t n) {
+    return !host || cudaMemcpy(host, dev, n * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess;
+}
+bool fetch_bf16(float *host, const bf16 *dev, size_t n) {
+    if (!host) return true;
+    std::vector<bf16> h(n);
+    if (n && cudaMemcpy(h.data(), dev, n * sizeof(bf16), cudaMemcpyDeviceToHost) != cudaSuccess) return false;
+    for (size_t i = 0; i < n; ++i) host[i] = __bfloat162float(h[i]);
+    return true;
+}
+
+int max_len(const int32_t *row_off, int n_utt) {
+    int m = 0;
+    for (int i = 0; i < n_utt; ++i) m = std::max(m, row_off[i + 1] - row_off[i]);
+    return m;
+}
+bool offsets_ok(const int32_t *row_off, int n_utt, int rows_total) {
+    if (!row_off || n_utt < 1 || row_off[0] < 0 || row_off[n_utt] > rows_total) return false;
+    for (int i = 0; i < n_utt; ++i)
+        if (row_off[i + 1] < row_off[i]) return false;
+    return true;
+}
+
+bool is_act_kind(int k) { return k == EPI_BIAS_RELU_ACT || k == EPI_BIAS_SILU_ACT || k == EPI_BIAS_ACT; }
+
+}  // namespace
+
+extern "C" {
+
+pk_status pk_kernel_gemm(int device, int path, int math, int cluster, int M, int N, int K, int epi_kind, int qcols, int ldo, float alpha,
+                         int in_place, const float *A, const float *W, const float *bias, const float *resid, float *out_f32,
+                         float *out_hi, float *out_lo, int64_t *guard_bad) {
+    if (path < 0 || path > 2 || epi_kind < EPI_BIAS_F32 || epi_kind > EPI_QKV_ACT || M < 1 || N < 1 || K < 1 || !A || !W) return PK_ERR_INVALID;
+    if (math != PK_MATH_BF16X3 && math != PK_MATH_BF16X1 && math != PK_MATH_FP32) return PK_ERR_INVALID;
+    if ((path == 0) != (math == PK_MATH_FP32)) return PK_ERR_INVALID;
+    if (path != 0 && K % 64 != 0) return PK_ERR_INVALID;
+    if (path == 2 && M > 128) return PK_ERR_INVALID;
+    if (cluster != 1 && (path != 1 || math != PK_MATH_BF16X3 || !gemm_tc_cluster_supported(N, epi_kind, cluster))) return PK_ERR_INVALID;
+    const bool qkv = epi_kind == EPI_QKV_ACT, glu = epi_kind == EPI_GLU_F32, resid_k = epi_kind == EPI_RESID_F32;
+    if (qkv && (path == 0 || qcols <= 0 || qcols % 16 != 0 || qcols >= N)) return PK_ERR_INVALID;
+    if (glu && (N & 1)) return PK_ERR_INVALID;
+    const int n_out = glu ? N / 2 : qkv ? N - qcols : N;    // columns of the [M, ldo] output
+    if (ldo < n_out || (resid_k && !resid) || (in_place && !resid_k)) return PK_ERR_INVALID;
+    // outputs: fp32 [M, ldo] (q [M, qcols] for QKV) and, for the act kinds off fp32 math, bf16 planes [M, ldo]
+    const bool planes = (is_act_kind(epi_kind) || qkv) && path != 0;
+    if ((!planes && !out_f32) || (planes && !out_hi) || (qkv && !out_f32)) return PK_ERR_INVALID;
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const size_t n_o = (size_t)M * ldo, n_f = qkv ? (size_t)M * qcols : n_o;
+    float *dA = cx.upload(A, (size_t)M * K), *dW = cx.upload(W, (size_t)N * K), *db = bias ? cx.upload(bias, N) : nullptr;
+    float *of = (planes && !qkv) ? nullptr : cx.guarded<float>(n_f);
+    bf16 *oh = planes ? cx.guarded<bf16>(n_o) : nullptr, *ol = planes && out_lo ? cx.guarded<bf16>(n_o) : nullptr;
+    float *dr = nullptr;
+    if (resid_k) {
+        if (in_place) {          // out_f32 starts as the residual and aliases it, as in pk_engine::gemm_ln
+            if (cudaMemcpy(of, resid, n_o * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) return PK_ERR_CUDA;
+            dr = of;
+        } else {
+            dr = cx.upload(resid, n_o);
+        }
+    }
+    if (!cx.ok) return PK_ERR_CUDA;
+    EpiParams ep;
+    ep.kind = epi_kind; ep.bias = db; ep.ldo = ldo; ep.resid = dr; ep.alpha = alpha; ep.qcols = qkv ? qcols : 0;
+    ep.out_f32 = of;
+    if (planes) { ep.act.hi = oh; ep.act.lo = ol; }
+    else if (is_act_kind(epi_kind)) ep.act.f32 = of;      // fp32 math: the activation is plain fp32
+    const bool split3 = math == PK_MATH_BF16X3;
+    if (path == 0) {
+        launch_gemm_simt(dA, K, dW, K, M, N, K, ep, cx.st);
+    } else {
+        bf16 *Ah = static_cast<bf16 *>(cx.alloc((size_t)M * K * 2)), *Al = static_cast<bf16 *>(cx.alloc((size_t)M * K * 2));
+        bf16 *Wh = static_cast<bf16 *>(cx.alloc((size_t)N * K * 2)), *Wl = static_cast<bf16 *>(cx.alloc((size_t)N * K * 2));
+        if (!cx.ok) return PK_ERR_CUDA;
+        ActBuf sa; sa.hi = Ah; sa.lo = Al;
+        ActBuf sw; sw.hi = Wh; sw.lo = Wl;
+        launch_split(dA, (size_t)M * K, sa, cx.st);
+        launch_split(dW, (size_t)N * K, sw, cx.st);
+        if (path == 2) {          // the few-row kernel, twice: its tickets must come back to zero
+            const size_t ws_floats = (size_t)2 << 20;
+            float *ws = static_cast<float *>(cx.alloc(ws_floats * sizeof(float)));
+            unsigned int *tk = static_cast<unsigned int *>(cx.alloc(1024 * sizeof(unsigned int)));
+            if (!cx.ok || cudaMemsetAsync(tk, 0, 1024 * sizeof(unsigned int), cx.st) != cudaSuccess) return PK_ERR_CUDA;
+            int sms = 0;
+            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+            for (int rep = 0; rep < 2; ++rep) {
+                // in place, the first launch has already added to the residual: start the second from it again
+                if (rep && in_place && cudaMemcpyAsync(of, resid, n_o * sizeof(float), cudaMemcpyHostToDevice, cx.st) != cudaSuccess)
+                    return PK_ERR_CUDA;
+                if (launch_gemm_skinny(Ah, Al, K, Wh, Wl, M, N, K, split3, ep, ws, ws_floats, tk, 1024, sms,
+                                       cx.st) != cudaSuccess)
+                    return PK_ERR_CUDA;
+            }
+            std::vector<unsigned int> htk(1024);
+            if (!cx.sync() || cudaMemcpy(htk.data(), tk, 1024 * sizeof(unsigned int), cudaMemcpyDeviceToHost) != cudaSuccess) return PK_ERR_CUDA;
+            for (unsigned int t : htk)
+                if (t != 0) return PK_ERR_CUDA;
+        } else {
+            TcOperand ta, tw, ta_sl;
+            if (!make_tc_operand(&ta, Ah, Al, M, K, 128) || !make_tc_operand(&tw, Wh, Wl, N, K, tc_tile_n(N)))
+                return PK_ERR_CUDA;
+            if (cluster > 1 && !make_tc_operand(&ta_sl, Ah, Al, M, K, 128 / cluster)) return PK_ERR_CUDA;
+            if (launch_gemm_tc(ta, tw, M, N, K, split3, ep, cx.st, cluster, cluster > 1 ? &ta_sl : nullptr) != cudaSuccess) return PK_ERR_CUDA;
+        }
+    }
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    if (of && !fetch_f32(out_f32, of, n_f)) return PK_ERR_CUDA;
+    if (oh && !fetch_bf16(out_hi, oh, n_o)) return PK_ERR_CUDA;
+    if (ol && !fetch_bf16(out_lo, ol, n_o)) return PK_ERR_CUDA;
+    return PK_OK;
+}
+
+pk_status pk_kernel_attention(int device, int kernel, int math, int n_utt, const int32_t *row_off, int rows_total, int d_model, int n_heads,
+                              int tmax, const float *qkv, const float *pp, const float *pos_u, const float *pos_v, float *ctx_f32,
+                              float *ctx_hi, float *ctx_lo, int64_t *guard_bad) {
+    if (kernel < 0 || kernel > 2 || !offsets_ok(row_off, n_utt, rows_total) || n_heads < 1 || d_model % n_heads || tmax < 1 || !qkv || !pp ||
+        !pos_u || !pos_v)
+        return PK_ERR_INVALID;
+    const int hd = d_model / n_heads, maxT = max_len(row_off, n_utt);
+    if (maxT > tmax || maxT < 1) return PK_ERR_INVALID;
+    if (kernel == 2 && !relpos_attention_wgmma_supported(hd, maxT)) return PK_ERR_INVALID;
+    // the output is what the engine's ctx buffer holds in that math mode: fp32, or bf16 hi (| lo) planes
+    const bool f32 = math == PK_MATH_FP32;
+    if (f32 ? (kernel != 0 || !ctx_f32) : (!ctx_hi || (math == PK_MATH_BF16X3) != (ctx_lo != nullptr))) return PK_ERR_INVALID;
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const int d = d_model, NP = 2 * tmax - 1;
+    const size_t n_o = (size_t)rows_total * d;
+    int32_t *doff = cx.upload(row_off, n_utt + 1);
+    float *dqkv = cx.upload(qkv, (size_t)rows_total * 3 * d), *dpp = cx.upload(pp, (size_t)NP * d);
+    float *du = cx.upload(pos_u, d), *dv = cx.upload(pos_v, d);
+    ActBuf out;
+    out.f32 = f32 ? cx.guarded<float>(n_o) : nullptr;
+    out.hi = f32 ? nullptr : cx.guarded<bf16>(n_o);
+    out.lo = ctx_lo ? cx.guarded<bf16>(n_o) : nullptr;
+    if (!cx.ok) return PK_ERR_CUDA;
+    bool launched;
+    if (kernel == 0) {
+        launched = launch_relpos_attention(dqkv, 3 * d, doff, n_utt, maxT, n_heads, hd, dpp, tmax, du, dv, d, out, cx.st);
+    } else {
+        // the EPI_QKV_ACT epilogue's layout: q fp32 [M, d], k | v bf16 planes [M, 2 d]; the position table split once at load
+        std::vector<float> hq((size_t)rows_total * d), hkv((size_t)rows_total * 2 * d);
+        for (int r = 0; r < rows_total; ++r) {
+            memcpy(&hq[(size_t)r * d], qkv + (size_t)r * 3 * d, (size_t)d * 4);
+            memcpy(&hkv[(size_t)r * 2 * d], qkv + (size_t)r * 3 * d + d, (size_t)2 * d * 4);
+        }
+        float *dq32 = cx.upload(hq.data(), hq.size()), *dkv = cx.upload(hkv.data(), hkv.size());
+        bf16 *kvh = static_cast<bf16 *>(cx.alloc(hkv.size() * 2)), *kvl = static_cast<bf16 *>(cx.alloc(hkv.size() * 2));
+        bf16 *pph = static_cast<bf16 *>(cx.alloc((size_t)NP * d * 2)), *ppl = static_cast<bf16 *>(cx.alloc((size_t)NP * d * 2));
+        if (!cx.ok) return PK_ERR_CUDA;
+        ActBuf skv; skv.hi = kvh; skv.lo = kvl;
+        ActBuf spp; spp.hi = pph; spp.lo = ppl;
+        launch_split(dkv, hkv.size(), skv, cx.st);
+        launch_split(dpp, (size_t)NP * d, spp, cx.st);
+        launched = kernel == 1
+                       ? launch_relpos_attention_tc(dq32, du, dv, kvh, kvl, 2 * d, doff, n_utt, maxT, n_heads, hd, pph, ppl, tmax, d, out, cx.st)
+                       : launch_relpos_attention_wgmma(dq32, du, dv, kvh, kvl, 2 * d, doff, n_utt, maxT, n_heads, hd, pph, ppl, tmax, d, out, cx.st);
+    }
+    if (!launched) return PK_ERR_INVALID;
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    if (out.f32 && !fetch_f32(ctx_f32, out.f32, n_o)) return PK_ERR_CUDA;
+    if (out.hi && !fetch_bf16(ctx_hi, out.hi, n_o)) return PK_ERR_CUDA;
+    if (out.lo && !fetch_bf16(ctx_lo, out.lo, n_o)) return PK_ERR_CUDA;
+    return PK_OK;
+}
+
+pk_status pk_kernel_layernorm(int device, int M, int d, const float *x, const float *w1, const float *b1, const float *w2, const float *b2,
+                              int want_f32, int planes, float *y1_f32, float *act_f32, float *hi, float *lo, int64_t *guard_bad) {
+    if (M < 1 || d < 128 || d > 1024 || d % 128 || !x || !w1 || !b1 || (!w2) != (!b2) || planes < 0 || planes > 3) return PK_ERR_INVALID;
+    if ((want_f32 && !y1_f32) || (planes == 3 && !act_f32) || ((planes == 1 || planes == 2) && !hi) || (planes == 2 && !lo)) return PK_ERR_INVALID;
+    if (w2 && (!want_f32 || planes == 0)) return PK_ERR_INVALID;    // the chained form: y1 in place, LN2(y1) as the operand
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const size_t n = (size_t)M * d;
+    float *dw1 = cx.upload(w1, d), *db1 = cx.upload(b1, d), *dw2 = w2 ? cx.upload(w2, d) : nullptr, *db2 = b2 ? cx.upload(b2, d) : nullptr;
+    float *y1 = want_f32 ? cx.guarded<float>(n) : nullptr;
+    float *dx;
+    if (y1) {                 // LN1 written in place over its input, as pk_engine::gemm_ln does
+        if (cudaMemcpy(y1, x, n * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) return PK_ERR_CUDA;
+        dx = y1;
+    } else {
+        dx = cx.upload(x, n);
+    }
+    ActBuf act;
+    if (planes == 3) act.f32 = cx.guarded<float>(n);
+    if (planes == 1 || planes == 2) act.hi = cx.guarded<bf16>(n);
+    if (planes == 2) act.lo = cx.guarded<bf16>(n);
+    if (!cx.ok) return PK_ERR_CUDA;
+    ActBuf none;
+    if (w2) launch_layernorm(dx, M, d, dw1, db1, y1, none, dw2, db2, act, cx.st);
+    else launch_layernorm(dx, M, d, dw1, db1, y1, act, nullptr, nullptr, none, cx.st);
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    if (!fetch_f32(y1 ? y1_f32 : nullptr, y1, n) || (act.f32 && !fetch_f32(act_f32, act.f32, n)) || (act.hi && !fetch_bf16(hi, act.hi, n)) ||
+        (act.lo && !fetch_bf16(lo, act.lo, n)))
+        return PK_ERR_CUDA;
+    return PK_OK;
+}
+
+pk_status pk_kernel_dwconv(int device, int math, int n_utt, const int32_t *row_off, int rows_total, int d, int ks, const float *g,
+                           const float *w_tapmajor, const float *bias, float *out_f32, float *hi, float *lo, int64_t *guard_bad) {
+    if (!offsets_ok(row_off, n_utt, rows_total) || d < 4 || d % 4 || ks < 1 || !g || !w_tapmajor || !bias) return PK_ERR_INVALID;
+    const bool f32 = math == PK_MATH_FP32;
+    if (f32 ? !out_f32 : (!hi || (math == PK_MATH_BF16X3) != (lo != nullptr))) return PK_ERR_INVALID;
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const size_t n = (size_t)rows_total * d;
+    int32_t *doff = cx.upload(row_off, n_utt + 1);
+    float *dg = cx.upload(g, n), *dw = cx.upload(w_tapmajor, (size_t)ks * d), *db = cx.upload(bias, d);
+    ActBuf out;
+    out.f32 = f32 ? cx.guarded<float>(n) : nullptr;
+    out.hi = f32 ? nullptr : cx.guarded<bf16>(n);
+    out.lo = lo ? cx.guarded<bf16>(n) : nullptr;
+    if (!cx.ok) return PK_ERR_CUDA;
+    if (!launch_dwconv_bn_silu(dg, doff, n_utt, max_len(row_off, n_utt), d, ks, dw, db, out, cx.st)) return PK_ERR_INVALID;
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    if ((out.f32 && !fetch_f32(out_f32, out.f32, n)) || (out.hi && !fetch_bf16(hi, out.hi, n)) || (out.lo && !fetch_bf16(lo, out.lo, n)))
+        return PK_ERR_CUDA;
+    return PK_OK;
+}
+
+pk_status pk_kernel_ctc_argmax(int device, int M, int V, int ld, const float *logits, int32_t *best, float *conf, float *logprobs,
+                               int64_t *guard_bad) {
+    if (M < 1 || V < 1 || ld < V || !logits || !best || !conf) return PK_ERR_INVALID;
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    float *dl = cx.upload(logits, (size_t)M * ld);
+    int32_t *db = cx.guarded<int32_t>(M);
+    float *dc = cx.guarded<float>(M), *dlp = logprobs ? cx.guarded<float>((size_t)M * V) : nullptr;
+    if (!cx.ok) return PK_ERR_CUDA;
+    launch_ctc_frame_argmax(dl, M, V, ld, db, dc, dlp, cx.st);
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    if (cudaMemcpy(best, db, (size_t)M * 4, cudaMemcpyDeviceToHost) != cudaSuccess || !fetch_f32(conf, dc, M) ||
+        (dlp && !fetch_f32(logprobs, dlp, (size_t)M * V)))
+        return PK_ERR_CUDA;
+    return PK_OK;
+}
+
+}  // extern "C"

@@ -45,7 +45,8 @@ EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_en
            "pk_mel_frames", "pk_encoder_frames", "pk_mel", "pk_encode", "pk_decode", "pk_ctc_logprobs",
            "pk_transcribe_batch", "pk_stage_pcm", "pk_prefetch_pcm", "pk_run_staged", "pk_fetch_tokens", "pk_sync",
            "pk_token_buffer", "pk_stream", "pk_launch_count", "pk_profile_begin", "pk_profile_end",
-           "pk_profile_names", "pk_flush_l2", "pk_selftest_gemm", "pk_selftest_gemm_ln", "pk_selftest_attention", "pk_debug_tdt_phases", "pk_vocab_load", "pk_vocab_free", "pk_vocab_size",
+           "pk_profile_names", "pk_flush_l2", "pk_selftest_gemm", "pk_selftest_gemm_ln", "pk_selftest_attention",
+           "pk_kernel_gemm", "pk_kernel_attention", "pk_kernel_layernorm", "pk_kernel_dwconv", "pk_kernel_ctc_argmax", "pk_debug_tdt_phases", "pk_vocab_load", "pk_vocab_free", "pk_vocab_size",
            "pk_detokenize", "pk_group_words", "pk_tokenize", "pk_ctc_decode_boosted",
            "pk_resample_len", "pk_resample",
            "pk_job_begin", "pk_job_append", "pk_nccl_unique_id", "pk_comm_init_rank", "pk_allgather_tokens",
@@ -109,6 +110,11 @@ def load_library():
     L.pk_selftest_gemm.argtypes = [C.c_int] * 6 + [C.c_uint32, f32p, f32p]
     L.pk_selftest_gemm_ln.argtypes = [C.c_int] * 5 + [C.c_uint32, f32p]
     L.pk_selftest_attention.argtypes = [C.c_int, i32p, C.c_int, C.c_int, C.c_int, C.c_uint32, f32p]
+    L.pk_kernel_gemm.argtypes = [C.c_int] * 10 + [C.c_float, C.c_int] + [f32p] * 7 + [i64p]
+    L.pk_kernel_attention.argtypes = [C.c_int] * 4 + [i32p] + [C.c_int] * 4 + [f32p] * 7 + [i64p]
+    L.pk_kernel_layernorm.argtypes = [C.c_int] * 3 + [f32p] * 5 + [C.c_int] * 2 + [f32p] * 4 + [i64p]
+    L.pk_kernel_dwconv.argtypes = [C.c_int] * 3 + [i32p] + [C.c_int] * 3 + [f32p] * 6 + [i64p]
+    L.pk_kernel_ctc_argmax.argtypes = [C.c_int] * 4 + [f32p, i32p, f32p, f32p, i64p]
     L.pk_vocab_load.argtypes = [C.c_char_p, C.POINTER(vp)]
     L.pk_vocab_free.argtypes = [vp]
     L.pk_vocab_size.argtypes = [vp]
