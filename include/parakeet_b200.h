@@ -293,6 +293,48 @@ pk_status pk_kernel_dwconv(int device, int math, int n_utt, const int32_t *row_o
 pk_status pk_kernel_ctc_argmax(int device, int M, int V, int ld, const float *logits, int32_t *best, float *conf, float *logprobs,
                                int64_t *guard_bad);
 
+/* The TDT / RNN-T decode kernel (csrc/tdt.cu) on host fp32 inputs in the reference's layouts, with the TdtParams that the engine
+ * builds: Bpad = n_utt rounded up to 32, LSTM weights reordered unit-major and split into bf16 hi/lo rows, the initial h split into
+ * state plane 0.  n_dur = 0 is an RNN-T joint (max_sym symbols per frame).  Utterance b = rows [row_off[b], row_off[b+1]) of EP. */
+typedef struct {
+    int32_t P, J, V, n_dur, durations[8], L, max_sym;
+    int32_t n_utt, rows;
+    const int32_t *row_off;                /* [n_utt + 1] */
+    const float *EP;                       /* [rows][J]   enc_proj(enc) + bias */
+    const float *G0;                       /* [V][4P]     W_ih0 . E[token] + b_ih0 */
+    const float *W_hh[4], *W_ih[4];        /* [4P][P] gate-major (i, f, g, o); W_ih for layers >= 1 */
+    const float *b_ih[4];                  /* [4P], layers >= 1 */
+    const float *W_p;                      /* [J][P] */
+    const float *W_out, *b_out;            /* [V + n_dur][J], [V + n_dur] */
+    int32_t cap, max_steps;
+    int32_t carry;                         /* 1: carried state (the streaming decode): the four arrays below are read */
+    const float *h0, *c0;                  /* [L][n_utt][P] committed LSTM state */
+    const int32_t *tok0, *frame_base;      /* [n_utt] last token, absolute frame of the first row */
+    int32_t cluster;                       /* 0 = the engine's choice, 2 / 4 = only that size (PK_ERR_INVALID if it does not fit) */
+    int32_t max_ctas;                      /* 0 = every SM, else the SM count the launch plans for */
+    int32_t no_stage;                      /* 1: no staging tile, as PK_TDT_NO_STAGE */
+} pk_tdt_hook_in;
+/* Outputs (every array guarded; NULL pointers are not fetched).  h, z and the keys are those of the LAST step: h_hi / h_lo
+ * [L][2][n_utt][P] are both state planes of every layer (the step's new h sits in the plane the utterance's committed state
+ * does not), z_hi / z_lo [n_utt][J]; lab_idx / dur_idx = -1 where no CTA posted a key (the utterance was idle, or no logit
+ * was above -inf); lse [n_utt] = the label log-sum-exp from that step's per-CTA (max, sum) partials, combined in double.
+ * With carry: c_state [L][n_utt][P], tok_state [n_utt] (h_hi / h_lo plane 0 holds the committed h). */
+typedef struct {
+    int32_t *tok;                          /* [n_utt][1 + cap]: len, ids */
+    int32_t *t_start, *t_end;              /* [n_utt][cap] */
+    float *t_conf;                         /* [n_utt][cap] */
+    int32_t *overflow;                     /* [n_utt] */
+    float *h_hi, *h_lo, *z_hi, *z_lo;
+    float *lab_val, *dur_val;              /* [n_utt] */
+    int32_t *lab_idx, *dur_idx;            /* [n_utt] */
+    double *lse;                           /* [n_utt] */
+    float *c_state;
+    int32_t *tok_state;
+    int32_t steps;
+    int32_t grid, cl, upc, opc, out_in_smem, wih_in_smem, staged_ih, wstage_rows;
+} pk_tdt_hook_out;
+pk_status pk_kernel_tdt_decode(int device, const pk_tdt_hook_in *in, pk_tdt_hook_out *out, int64_t *guard_bad);
+
 /* Host-side text helpers (pure C++ host code; no device work):
  * Tokenizer::load/decode (src/vocab.cpp:10-64), group_timestamps (src/timestamp.cpp:24-75). */
 typedef struct pk_vocab pk_vocab;

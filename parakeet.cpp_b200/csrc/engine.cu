@@ -305,9 +305,7 @@ pk_status pk_engine::load(const char *path) {
                 std::vector<float> src, dst((size_t)4 * P * P);
                 for (int which = 0; which < 2; ++which) {
                     if (!st.read_f32(q + (which ? "input_proj_.weight" : "hidden_proj_.weight"), src, (int64_t)4 * P * P, e)) return fail(PK_ERR_MISSING, e);
-                    for (int u = 0; u < P; ++u)
-                        for (int gt = 0; gt < 4; ++gt)
-                            memcpy(&dst[((size_t)u * 4 + gt) * P], &src[((size_t)gt * P + u) * P], (size_t)P * sizeof(float));
+                    lstm_unit_major(src.data(), P, dst.data());
                     float *d = upload(dst);
                     if (!d) return fail(PK_ERR_CUDA, "cudaMalloc failed (LSTM weights)");
                     (which ? Wih_um[l] : Whh_um[l]) = d;

@@ -6,6 +6,7 @@
 // kernel must not write come back still holding the pattern, so the caller can check the exact set of written elements.
 // bf16 planes come back widened to fp32 (exact).  A private stream, synchronous; nothing is cached between calls.
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <vector>
 
@@ -321,6 +322,163 @@ pk_status pk_kernel_ctc_argmax(int device, int M, int V, int ld, const float *lo
     if (cudaMemcpy(best, db, (size_t)M * 4, cudaMemcpyDeviceToHost) != cudaSuccess || !fetch_f32(conf, dc, M) ||
         (dlp && !fetch_f32(logprobs, dlp, (size_t)M * V)))
         return PK_ERR_CUDA;
+    return PK_OK;
+}
+
+pk_status pk_kernel_tdt_decode(int device, const pk_tdt_hook_in *in, pk_tdt_hook_out *out, int64_t *guard_bad) {
+    if (!in || !out) return PK_ERR_INVALID;
+    const int P = in->P, J = in->J, V = in->V, D = in->n_dur, L = in->L, n = in->n_utt;
+    if (P < 32 || P % 32 || J < 32 || J % 32 || V < 2 || D < 0 || D > 8 || L < 1 || L > PK_MAX_LSTM || n < 1 || in->cap < 1 ||
+        in->max_steps < 1 || (D == 0 && in->max_sym < 1) || !offsets_ok(in->row_off, n, in->rows) || !in->EP || !in->G0 || !in->W_p ||
+        !in->W_out || !in->b_out || (in->cluster != 0 && in->cluster != 2 && in->cluster != 4) || in->max_ctas < 0)
+        return PK_ERR_INVALID;
+    for (int l = 0; l < L; ++l)
+        if (!in->W_hh[l] || (l > 0 && (!in->W_ih[l] || !in->b_ih[l]))) return PK_ERR_INVALID;
+    if (in->carry && (!in->h0 || !in->c0 || !in->tok0 || !in->frame_base)) return PK_ERR_INVALID;
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const int Bpad = (n + 31) / 32 * 32, cap = in->cap, NO = V + D;
+    const size_t HS = (size_t)P * Bpad;
+    TdtParams p{};
+    p.P = P; p.J = J; p.V = V; p.D = D; p.L = L; p.Bpad = Bpad; p.n_utt = n; p.cap = cap; p.max_steps = in->max_steps;
+    p.n_dur = D; p.max_sym = in->max_sym;
+    for (int i = 0; i < 8; ++i) p.durations[i] = in->durations[i];
+    p.EP = cx.upload(in->EP, (size_t)in->rows * J);
+    p.row_off = cx.upload(in->row_off, n + 1);
+    p.G0 = cx.upload(in->G0, (size_t)V * 4 * P);
+    // weights as the engine loads them: unit-major LSTM rows, every matrix split into [hi: K][lo: K] bf16 rows
+    auto split = [&](const float *w, int rows, int K) {
+        float *dw = cx.upload(w, (size_t)rows * K);
+        bf16 *s = static_cast<bf16 *>(cx.alloc((size_t)rows * 2 * K * sizeof(bf16)));
+        if (s) launch_tdt_split_rows(dw, rows, K, s, cx.st);
+        return static_cast<const bf16 *>(s);
+    };
+    std::vector<float> um((size_t)4 * P * P);
+    for (int l = 0; l < L; ++l) {
+        lstm_unit_major(in->W_hh[l], P, um.data());
+        p.Whh[l] = split(um.data(), 4 * P, P);
+        if (l > 0) {
+            lstm_unit_major(in->W_ih[l], P, um.data());
+            p.Wih[l] = split(um.data(), 4 * P, P);
+            p.bih[l] = cx.upload(in->b_ih[l], (size_t)4 * P);
+        }
+    }
+    p.Wp = split(in->W_p, J, P);
+    p.Wout = split(in->W_out, NO, J);
+    p.bout = cx.upload(in->b_out, NO);
+    // h: bf16 [hi|lo][L][2][Bpad][P], zero except the carried state in plane 0
+    bf16 *hb = cx.guarded<bf16>(2 * L * 2 * HS);
+    bf16 *zb = cx.guarded<bf16>((size_t)2 * Bpad * J);
+    {
+        std::vector<float> h((size_t)L * 2 * HS, 0.f);
+        if (in->carry)
+            for (int l = 0; l < L; ++l)
+                for (int b = 0; b < n; ++b) memcpy(&h[(size_t)l * 2 * HS + (size_t)b * P], in->h0 + ((size_t)l * n + b) * P, (size_t)P * 4);
+        float *dh = cx.upload(h.data(), h.size());
+        if (!cx.ok) return PK_ERR_CUDA;
+        ActBuf sh; sh.hi = hb; sh.lo = hb + (size_t)L * 2 * HS;
+        launch_split(dh, h.size(), sh, cx.st);
+    }
+    p.hbuf = reinterpret_cast<float *>(hb);
+    p.z = reinterpret_cast<float *>(zb);
+    p.tok = cx.guarded<int32_t>((size_t)n * (1 + cap));
+    p.t_start = cx.guarded<int32_t>((size_t)n * cap);
+    p.t_end = cx.guarded<int32_t>((size_t)n * cap);
+    p.t_conf = cx.guarded<float>((size_t)n * cap);
+    p.overflow = cx.guarded<int32_t>(n);
+    constexpr int kMaxGrid = 256;           // launch_tdt_decode never plans a larger grid
+    p.pl_max = static_cast<float *>(cx.alloc((size_t)3 * kMaxGrid * Bpad * sizeof(float)));
+    p.pl_sum = static_cast<float *>(cx.alloc((size_t)3 * kMaxGrid * Bpad * sizeof(float)));
+    p.key_lab = static_cast<unsigned long long *>(cx.alloc((size_t)3 * Bpad * 8));
+    p.key_dur = static_cast<unsigned long long *>(cx.alloc((size_t)3 * Bpad * 8));
+    p.bar = static_cast<unsigned int *>(cx.alloc(1024 * sizeof(unsigned int)));
+    p.dbg = static_cast<long long *>(cx.alloc(8 * sizeof(long long)));
+    if (in->carry) {
+        p.carry = 1;
+        std::vector<float> c((size_t)L * Bpad * P, 0.f);
+        for (int l = 0; l < L; ++l)
+            memcpy(&c[(size_t)l * Bpad * P], in->c0 + (size_t)l * n * P, (size_t)n * P * 4);
+        p.c_state = cx.guarded<float>(c.size());
+        p.tok_state = cx.guarded<int32_t>(n);
+        p.frame_base = cx.upload(in->frame_base, n);
+        if (!cx.ok || cudaMemcpy(p.c_state, c.data(), c.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
+            cudaMemcpy(p.tok_state, in->tok0, (size_t)n * 4, cudaMemcpyHostToDevice) != cudaSuccess)
+            return PK_ERR_CUDA;
+    }
+    if (!cx.ok || !cx.sync()) return PK_ERR_CUDA;
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    TdtLaunchCtl ctl;
+    ctl.cluster = in->cluster;
+    ctl.no_stage = in->no_stage != 0;
+    const cudaError_t ce = launch_tdt_decode(p, in->max_ctas ? std::min(in->max_ctas, sms) : sms, cx.st, &ctl);
+    if (ce == cudaErrorLaunchOutOfResources && ctl.grid == 0) {
+        cudaGetLastError();
+        return PK_ERR_INVALID;               // (a forced cluster size that does not fit)
+    }
+    if (ce != cudaSuccess) return PK_ERR_CUDA;
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    out->grid = ctl.grid; out->cl = ctl.CL; out->upc = ctl.UPC; out->opc = ctl.OPC;
+    out->out_in_smem = ctl.out_in_smem; out->wih_in_smem = ctl.wih_in_smem; out->staged_ih = ctl.staged_ih; out->wstage_rows = ctl.wstage_rows;
+    long long dbg[8];
+    if (cudaMemcpy(dbg, p.dbg, sizeof(dbg), cudaMemcpyDeviceToHost) != cudaSuccess) return PK_ERR_CUDA;
+    out->steps = (int32_t)dbg[7];
+    const int kb = (out->steps - 1) % 3, G = ctl.grid;
+    auto fetch_i32 = [](int32_t *host, const int32_t *dev, size_t cnt) {
+        return !host || cudaMemcpy(host, dev, cnt * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
+    };
+    if (!fetch_i32(out->tok, p.tok, (size_t)n * (1 + cap)) || !fetch_i32(out->t_start, p.t_start, (size_t)n * cap) ||
+        !fetch_i32(out->t_end, p.t_end, (size_t)n * cap) || !fetch_f32(out->t_conf, p.t_conf, (size_t)n * cap) ||
+        !fetch_i32(out->overflow, p.overflow, n))
+        return PK_ERR_CUDA;
+    // h planes and z: drop the batch padding rows
+    for (int pl = 0; pl < 2; ++pl) {
+        float *dst = pl ? out->h_lo : out->h_hi;
+        if (dst)
+            for (int s = 0; s < L * 2; ++s)
+                if (!fetch_bf16(dst + (size_t)s * n * P, hb + (size_t)pl * L * 2 * HS + (size_t)s * HS, (size_t)n * P)) return PK_ERR_CUDA;
+        float *zd = pl ? out->z_lo : out->z_hi;
+        if (!fetch_bf16(zd, zb + (size_t)pl * Bpad * J, (size_t)n * J)) return PK_ERR_CUDA;
+    }
+    std::vector<unsigned long long> keys(2 * (size_t)Bpad);
+    std::vector<float> pm((size_t)G * Bpad), ps((size_t)G * Bpad);
+    if (cudaMemcpy(keys.data(), p.key_lab + (size_t)kb * Bpad, (size_t)Bpad * 8, cudaMemcpyDeviceToHost) != cudaSuccess ||
+        cudaMemcpy(keys.data() + Bpad, p.key_dur + (size_t)kb * Bpad, (size_t)Bpad * 8, cudaMemcpyDeviceToHost) != cudaSuccess ||
+        cudaMemcpy(pm.data(), p.pl_max + (size_t)kb * G * Bpad, pm.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess ||
+        cudaMemcpy(ps.data(), p.pl_sum + (size_t)kb * G * Bpad, ps.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess)
+        return PK_ERR_CUDA;
+    for (int b = 0; b < n; ++b) {
+        for (int which = 0; which < 2; ++which) {     // the packing of tdt.cu's pack_key
+            const unsigned long long k = keys[(size_t)which * Bpad + b];
+            uint32_t u = (uint32_t)(k >> 32);
+            u = (u & 0x80000000u) ? (u & 0x7FFFFFFFu) : ~u;
+            float v;
+            memcpy(&v, &u, 4);
+            const int32_t idx = k ? (int32_t)(0xFFFFFFFFu - (uint32_t)(k & 0xFFFFFFFFu)) : -1;
+            if (which == 0) {
+                if (out->lab_val) out->lab_val[b] = v;
+                if (out->lab_idx) out->lab_idx[b] = idx;
+            } else {
+                if (out->dur_val) out->dur_val[b] = v;
+                if (out->dur_idx) out->dur_idx[b] = idx;
+            }
+        }
+        if (out->lse) {
+            double gmax = -INFINITY, s = 0.0;
+            for (int q = 0; q < G; ++q) gmax = std::max(gmax, (double)pm[(size_t)q * Bpad + b]);
+            for (int q = 0; q < G; ++q)
+                if (pm[(size_t)q * Bpad + b] > -INFINITY) s += (double)ps[(size_t)q * Bpad + b] * std::exp((double)pm[(size_t)q * Bpad + b] - gmax);
+            out->lse[b] = gmax + std::log(s);
+        }
+    }
+    if (in->carry) {
+        std::vector<float> c((size_t)L * Bpad * P);
+        if (cudaMemcpy(c.data(), p.c_state, c.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess || !fetch_i32(out->tok_state, p.tok_state, n))
+            return PK_ERR_CUDA;
+        if (out->c_state)
+            for (int l = 0; l < L; ++l) memcpy(out->c_state + (size_t)l * n * P, &c[(size_t)l * Bpad * P], (size_t)n * P * 4);
+    }
     return PK_OK;
 }
 

@@ -54,6 +54,7 @@
 // are fetched BEFORE the product so their L2 latency overlaps it; the LSTM cell state never leaves
 // shared memory.
 #include <cstdlib>
+#include <cstring>
 
 #include "kernels.h"
 
@@ -326,11 +327,13 @@ __device__ __forceinline__ unsigned long long pack_key(float v, int idx) {
     u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
     return ((unsigned long long)u << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned int)idx);
 }
+// k = 0 is a key no CTA posted: no logit above -inf.  Its index is 0, as the reference's strict '>' scan from index 0
+// (and the oracle's first_argmax) gives; the value is then meaningless.
 __device__ __forceinline__ void unpack_key(unsigned long long k, float &v, int &idx) {
     unsigned int u = (unsigned int)(k >> 32);
     u = (u & 0x80000000u) ? (u & 0x7FFFFFFFu) : ~u;
     v = __uint_as_float(u);
-    idx = (int)(0xFFFFFFFFu - (unsigned int)(k & 0xFFFFFFFFu));
+    idx = k ? (int)(0xFFFFFFFFu - (unsigned int)(k & 0xFFFFFFFFu)) : 0;
 }
 
 struct TdtGeom {            // per-cluster row blocks and per-CTA shared-memory sizes (host and device agree)
@@ -867,7 +870,7 @@ size_t tdt_smem_bytes(const TdtParams &p, int n_clusters, int CL, bool *out_in_s
 }
 
 template <int CL>
-cudaError_t launch_cl(TdtParams p, int num_sms, cudaStream_t st, bool *fits) {
+cudaError_t launch_cl(TdtParams p, int num_sms, cudaStream_t st, bool *fits, TdtLaunchCtl *ctl) {
     *fits = false;
     if (p.P % (16 * CL) || p.J % (16 * CL)) return cudaSuccess;
     // upper bound on clusters; the occupancy query below says how many can be co-resident
@@ -902,8 +905,15 @@ cudaError_t launch_cl(TdtParams p, int num_sms, cudaStream_t st, bool *fits) {
             p.out_in_smem = out_in_smem ? 1 : 0;
             p.wih_in_smem = wih_in_smem ? 1 : 0;
             p.smem_lstm_floats = lstm_floats;
-            p.wstage_rows = getenv("PK_TDT_NO_STAGE") ? 0 : wstage_rows;
+            p.wstage_rows = (getenv("PK_TDT_NO_STAGE") || (ctl && ctl->no_stage)) ? 0 : wstage_rows;
             *fits = true;
+            if (ctl) {
+                const TdtGeom ge = tdt_geom(p.P, p.J, p.V + p.D, nc, CL);
+                const int nU0 = ge.UPC < p.P ? ge.UPC : p.P;          // units of cluster 0 (the kernel's staged_ih, per cluster)
+                ctl->grid = nc * CL; ctl->CL = CL; ctl->UPC = ge.UPC; ctl->OPC = ge.OPC;
+                ctl->out_in_smem = p.out_in_smem; ctl->wih_in_smem = p.wih_in_smem; ctl->wstage_rows = p.wstage_rows;
+                ctl->staged_ih = !p.wih_in_smem && p.L > 1 && p.wstage_rows >= nU0 * 4 && nU0 <= RG / 4 && ge.KSP == ge.KSJ;
+            }
             tdt_init_kernel<<<((3 * p.Bpad > GBAR * GBAR_STRIDE ? 3 * p.Bpad : GBAR * GBAR_STRIDE) + 127) / 128, 128, 0, st>>>(p);
             return cudaLaunchKernelEx(&cfg, tdt_decode_kernel<CL>, p);
         }
@@ -912,10 +922,6 @@ cudaError_t launch_cl(TdtParams p, int num_sms, cudaStream_t st, bool *fits) {
     }
     return cudaSuccess;
 }
-
-// Co-resident cluster counts are a property of the device and the kernel's footprint: decide once
-// which cluster size to use (prefer 4 when it keeps >= 3/4 of the SMs busy).
-int g_tdt_cl = 0;
 
 }  // namespace
 
@@ -931,21 +937,28 @@ void launch_tdt_split_rows(const float *src, int rows, int K, bf16 *dst, cudaStr
     tdt_split_rows_kernel<<<256, 256, 0, st>>>(src, rows, K, dst);
 }
 
-cudaError_t launch_tdt_decode(TdtParams p, int num_sms, cudaStream_t st) {
+cudaError_t launch_tdt_decode(TdtParams p, int num_sms, cudaStream_t st, TdtLaunchCtl *ctl) {
+    // The cluster size is decided for every launch from its shapes and the occupancy query: 4 where it fits, else 2.
+    int cl = 4;
+    if (ctl && ctl->cluster) cl = ctl->cluster;
+    else if (const char *ev = getenv("PK_TDT_CLUSTER")) cl = atoi(ev) == 2 ? 2 : 4;
+    const bool fallback = !(ctl && ctl->cluster);
+    if (ctl) ctl->grid = 0;
     bool fits = false;
     cudaError_t err;
-    if (g_tdt_cl == 0) {
-        g_tdt_cl = 4;
-        if (const char *ev = getenv("PK_TDT_CLUSTER")) g_tdt_cl = atoi(ev) == 2 ? 2 : 4;
-    }
-    if (g_tdt_cl == 4) {
-        err = launch_cl<4>(p, num_sms, st, &fits);
+    if (cl == 4) {
+        err = launch_cl<4>(p, num_sms, st, &fits, ctl);
         if (fits) return err;
-        g_tdt_cl = 2;
+        if (!fallback) return cudaErrorLaunchOutOfResources;
     }
-    err = launch_cl<2>(p, num_sms, st, &fits);
+    err = launch_cl<2>(p, num_sms, st, &fits, ctl);
     if (fits) return err;
     return cudaErrorLaunchOutOfResources;
+}
+
+void lstm_unit_major(const float *src, int P, float *dst) {
+    for (int u = 0; u < P; ++u)
+        for (int gt = 0; gt < 4; ++gt) memcpy(&dst[((size_t)u * 4 + gt) * P], &src[((size_t)gt * P + u) * P], (size_t)P * sizeof(float));
 }
 
 }  // namespace pk

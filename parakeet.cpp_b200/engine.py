@@ -41,12 +41,34 @@ class _PkTokens(C.Structure):
                 ("end", C.POINTER(C.c_int32)), ("conf", C.POINTER(C.c_float)), ("len", C.POINTER(C.c_int32))]
 
 
+class TdtHookIn(C.Structure):
+    """pk_tdt_hook_in (include/parakeet_b200.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("P", "J", "V", "n_dur")] + [("durations", C.c_int32 * 8)] + \
+        [(n, C.c_int32) for n in ("L", "max_sym", "n_utt", "rows")] + \
+        [("row_off", C.POINTER(C.c_int32)), ("EP", C.POINTER(C.c_float)), ("G0", C.POINTER(C.c_float)),
+         ("W_hh", C.POINTER(C.c_float) * 4), ("W_ih", C.POINTER(C.c_float) * 4), ("b_ih", C.POINTER(C.c_float) * 4),
+         ("W_p", C.POINTER(C.c_float)), ("W_out", C.POINTER(C.c_float)), ("b_out", C.POINTER(C.c_float)),
+         ("cap", C.c_int32), ("max_steps", C.c_int32), ("carry", C.c_int32),
+         ("h0", C.POINTER(C.c_float)), ("c0", C.POINTER(C.c_float)), ("tok0", C.POINTER(C.c_int32)),
+         ("frame_base", C.POINTER(C.c_int32)), ("cluster", C.c_int32), ("max_ctas", C.c_int32), ("no_stage", C.c_int32)]
+
+
+class TdtHookOut(C.Structure):
+    """pk_tdt_hook_out (include/parakeet_b200.h)."""
+    _fields_ = [("tok", C.POINTER(C.c_int32)), ("t_start", C.POINTER(C.c_int32)), ("t_end", C.POINTER(C.c_int32)),
+                ("t_conf", C.POINTER(C.c_float)), ("overflow", C.POINTER(C.c_int32))] + \
+        [(n, C.POINTER(C.c_float)) for n in ("h_hi", "h_lo", "z_hi", "z_lo", "lab_val", "dur_val")] + \
+        [("lab_idx", C.POINTER(C.c_int32)), ("dur_idx", C.POINTER(C.c_int32)), ("lse", C.POINTER(C.c_double)),
+         ("c_state", C.POINTER(C.c_float)), ("tok_state", C.POINTER(C.c_int32))] + \
+        [(n, C.c_int32) for n in ("steps", "grid", "cl", "upc", "opc", "out_in_smem", "wih_in_smem", "staged_ih", "wstage_rows")]
+
+
 EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_engine_create", "pk_engine_destroy", "pk_last_error",
            "pk_mel_frames", "pk_encoder_frames", "pk_mel", "pk_encode", "pk_decode", "pk_ctc_logprobs",
            "pk_transcribe_batch", "pk_stage_pcm", "pk_prefetch_pcm", "pk_run_staged", "pk_fetch_tokens", "pk_sync",
            "pk_token_buffer", "pk_stream", "pk_launch_count", "pk_profile_begin", "pk_profile_end",
            "pk_profile_names", "pk_flush_l2", "pk_selftest_gemm", "pk_selftest_gemm_ln", "pk_selftest_attention",
-           "pk_kernel_gemm", "pk_kernel_attention", "pk_kernel_layernorm", "pk_kernel_dwconv", "pk_kernel_ctc_argmax", "pk_debug_tdt_phases", "pk_vocab_load", "pk_vocab_free", "pk_vocab_size",
+           "pk_kernel_gemm", "pk_kernel_attention", "pk_kernel_layernorm", "pk_kernel_dwconv", "pk_kernel_ctc_argmax", "pk_kernel_tdt_decode", "pk_debug_tdt_phases", "pk_vocab_load", "pk_vocab_free", "pk_vocab_size",
            "pk_detokenize", "pk_group_words", "pk_tokenize", "pk_ctc_decode_boosted",
            "pk_resample_len", "pk_resample",
            "pk_job_begin", "pk_job_append", "pk_nccl_unique_id", "pk_comm_init_rank", "pk_allgather_tokens",
@@ -115,6 +137,7 @@ def load_library():
     L.pk_kernel_layernorm.argtypes = [C.c_int] * 3 + [f32p] * 5 + [C.c_int] * 2 + [f32p] * 4 + [i64p]
     L.pk_kernel_dwconv.argtypes = [C.c_int] * 3 + [i32p] + [C.c_int] * 3 + [f32p] * 6 + [i64p]
     L.pk_kernel_ctc_argmax.argtypes = [C.c_int] * 4 + [f32p, i32p, f32p, f32p, i64p]
+    L.pk_kernel_tdt_decode.argtypes = [C.c_int, C.POINTER(TdtHookIn), C.POINTER(TdtHookOut), i64p]
     L.pk_vocab_load.argtypes = [C.c_char_p, C.POINTER(vp)]
     L.pk_vocab_free.argtypes = [vp]
     L.pk_vocab_size.argtypes = [vp]
