@@ -1,5 +1,5 @@
 // tc_prims.cuh -- the sm_90a primitives of the wgmma GEMM kernels (gemm_tc.cu): mbarrier, TMA loads (plain and
-// multicast), thread-block cluster helpers, wgmma shared-memory descriptors, issue / commit / wait.
+// multicast) and stores, thread-block cluster helpers, wgmma shared-memory descriptors, issue / commit / wait.
 #pragma once
 #include <cuda.h>
 
@@ -21,8 +21,8 @@ __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
+// addr: the shared-memory address of the mbarrier
+__device__ __forceinline__ void mbar_wait(uint32_t addr, uint32_t parity) {
     uint32_t done = 0;
     for (uint32_t spin = 0; !done; ++spin) {
         asm volatile(
@@ -35,6 +35,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
         if (spin > (1u << 26)) __trap();   // ~seconds: protocol error, fail instead of hanging
     }
 }
+__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) { mbar_wait(smem_u32(bar), parity); }
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
@@ -56,6 +57,22 @@ __device__ __forceinline__ void tma_load_2d_mcast(void *smem_dst, const CUtensor
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0), "r"(c1), "l"(policy)
         : "memory");
 }
+// TMA store of one box from shared memory (tracked by the issuing thread's bulk async-groups), and the group operations:
+// commit the stores issued so far as one group; wait until at most N groups are still reading shared memory (.read) or
+// still writing global memory.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap *tm, uint32_t smem_src, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_src), "r"(c0), "r"(c1)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// makes this thread's shared-memory writes visible to the async proxy (a TMA store that reads them)
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
