@@ -81,6 +81,12 @@ typedef struct pk_engine pk_engine;
 void pk_config_110m(pk_config *cfg);      /* config.hpp:77-95  */
 void pk_config_tdt_600m(pk_config *cfg);  /* config.hpp:98-116 */
 void pk_config_rnnt_600m(pk_config *cfg); /* config.hpp:118-135 (mel 80, vocab 1025, n_durations = 0) */
+/* make_nemotron_600m_config (nemotron.hpp:33-54): the multilingual STREAMING model, opened with pk_stream_open.
+ * d 1024, 24 layers, 8 heads, ff 4096, 80 mels (the preset leaves mel_bins at its default), vocab 8193, 2 LSTM
+ * layers, TDT durations {0..4}, keys "encoder_." / "prediction_." / "joint_." (has_ctc 0, joint_prefix_tdt 0).
+ * Capacity suits streaming: max_batch 64 streams, max_samples 102400 (81 encoder frames >= left context 70 + the
+ * frames of one chunk).  The latency mode (att_context_right) is an argument of pk_stream_open, not of pk_config. */
+void pk_config_nemotron_600m(pk_config *cfg);
 
 /* Replaces Transcriber::Transcriber + to_gpu (transcribe.hpp:59-71):
  * safetensors::load (axiom io_safetensors.cpp:123-160) + load_state_dict(strict=false)
@@ -334,6 +340,25 @@ typedef struct {
     int32_t grid, cl, upc, opc, out_in_smem, wih_in_smem, staged_ih, wstage_rows;
 } pk_tdt_hook_out;
 pk_status pk_kernel_tdt_decode(int device, const pk_tdt_hook_in *in, pk_tdt_hook_out *out, int64_t *guard_bad);
+/* Streaming kernels as pk_stream_step launches them for one layer.  n_active of n_streams streams take part:
+ * act_stream[a] is stream a's id, its rows are [row_off[a], row_off[a+1]) of the packed step (rows_total in all).
+ * Per-stream state is indexed by stream id and updated in place; the updated state comes back in the *_out arrays.
+ * pk_kernel_stream_attention: cached attention (streaming_encoder.cpp:160-272) of qkv [rows_total][3 d] (q | k | v),
+ *   keys = [ring rows (oldest first) | the chunk's rows]; the ring of stream s is kc/vc [s][L][d] holding cache_len[s] rows
+ *   from slot ring_start[s] on (mod L); pp [(2 tmax - 1)][d] the projected position table, pos_u / pos_v [d].  Needs
+ *   L + max chunk rows <= tmax.  Output ctx [rows_total][d]: ctx_f32 with PK_MATH_FP32, else hi and, with
+ *   PK_MATH_BF16X3, lo; kc_out / vc_out [n_streams][L][d] the rings after the chunk's rows went in.
+ * pk_kernel_stream_dwconv: cached causal depthwise conv + folded BatchNorm + SiLU (streaming_encoder.cpp:41-80) of
+ *   glu [rows_total][d]; w [d][ks] (channel-major), bias [d]; cache [n_streams][ks - 1][d] the last ks - 1 inputs of
+ *   every stream.  Output as above; cache_out [n_streams][ks - 1][d]. */
+pk_status pk_kernel_stream_attention(int device, int math, int n_streams, int n_active, const int32_t *act_stream, const int32_t *row_off,
+                                     int rows_total, const int32_t *cache_len, const int32_t *ring_start, int L, int d_model, int n_heads,
+                                     int tmax, const float *qkv, const float *pp, const float *pos_u, const float *pos_v, const float *kc,
+                                     const float *vc, float *ctx_f32, float *ctx_hi, float *ctx_lo, float *kc_out, float *vc_out,
+                                     int64_t *guard_bad);
+pk_status pk_kernel_stream_dwconv(int device, int math, int n_streams, int n_active, const int32_t *act_stream, const int32_t *row_off,
+                                  int rows_total, int d, int ks, const float *glu, const float *w, const float *bias, const float *cache,
+                                  float *out_f32, float *hi, float *lo, float *cache_out, int64_t *guard_bad);
 
 /* Host-side text helpers (pure C++ host code; no device work):
  * Tokenizer::load/decode (src/vocab.cpp:10-64), group_timestamps (src/timestamp.cpp:24-75). */

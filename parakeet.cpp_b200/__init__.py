@@ -12,4 +12,5 @@ drop-in shim with the reference's class signatures is include/parakeet/transcrib
 from .engine import (Decoder, Engine, ModelConfig, TranscribeOptions, TranscribeResult, Transcriber,  # noqa: F401
                      TimestampedToken, WordTimestamp, lib_path, load_library, make_110m_config,
                      make_tdt_600m_config, make_tiny_config, make_eou_120m_config, make_tiny_stream_config,
-                     make_rnnt_600m_config, make_tiny_rnnt_config)
+                     make_rnnt_600m_config, make_tiny_rnnt_config, make_nemotron_600m_config,
+                     make_tiny_nemotron_config)

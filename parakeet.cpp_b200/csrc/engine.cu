@@ -869,6 +869,12 @@ void pk_config_rnnt_600m(pk_config *c) {
     c->has_ctc = 0; c->joint_prefix_tdt = 0; c->max_symbols = 10; c->max_batch = 16; c->max_samples = 480000;
 }
 
+void pk_config_nemotron_600m(pk_config *c) {
+    pk_config_110m(c);
+    c->d_model = 1024; c->n_layers = 24; c->ff = 4096; c->vocab = 8193; c->lstm_layers = 2;
+    c->has_ctc = 0; c->joint_prefix_tdt = 0; c->max_symbols = 10; c->max_batch = 64; c->max_samples = 102400;
+}
+
 int32_t pk_mel_frames(int64_t n_samples) { return (int32_t)(1 + n_samples / 160); }
 int32_t pk_encoder_frames(int32_t f) { return conv_len(conv_len(conv_len(f))); }
 

@@ -483,3 +483,101 @@ pk_status pk_kernel_tdt_decode(int device, const pk_tdt_hook_in *in, pk_tdt_hook
 }
 
 }  // extern "C"
+
+namespace {
+
+// the active-stream list of a streaming hook: distinct ids in [0, n_streams), row offsets over rows_total
+bool streams_ok(int n_streams, int n_active, const int32_t *act, const int32_t *row_off, int rows_total) {
+    if (n_streams < 1 || n_active < 1 || n_active > n_streams || !act || !offsets_ok(row_off, n_active, rows_total)) return false;
+    std::vector<char> seen(n_streams, 0);
+    for (int a = 0; a < n_active; ++a) {
+        if (act[a] < 0 || act[a] >= n_streams || seen[act[a]]) return false;
+        seen[act[a]] = 1;
+    }
+    return true;
+}
+
+// ctx / conv output in the engine's layout for the math mode: fp32, or bf16 hi (| lo) planes
+bool act_out_ok(int math, const float *f32, const float *hi, const float *lo) {
+    if (math == PK_MATH_FP32) return f32 != nullptr;
+    if (math != PK_MATH_BF16X3 && math != PK_MATH_BF16X1) return false;
+    return hi && (math == PK_MATH_BF16X3) == (lo != nullptr);
+}
+
+ActBuf guarded_act(HookCtx &cx, int math, size_t n, bool lo) {
+    ActBuf o;
+    if (math == PK_MATH_FP32) o.f32 = cx.guarded<float>(n);
+    else o.hi = cx.guarded<bf16>(n);
+    if (lo) o.lo = cx.guarded<bf16>(n);
+    return o;
+}
+
+bool fetch_act(const ActBuf &o, float *f32, float *hi, float *lo, size_t n) {
+    return (!o.f32 || fetch_f32(f32, o.f32, n)) && (!o.hi || fetch_bf16(hi, o.hi, n)) && (!o.lo || fetch_bf16(lo, o.lo, n));
+}
+
+// a guarded copy of host state (rings, conv caches) that the kernel updates in place
+float *guarded_state(HookCtx &cx, const float *h, size_t n) {
+    float *d = cx.guarded<float>(n);
+    if (d && cudaMemcpy(d, h, n * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) cx.ok = false;
+    return d;
+}
+
+}  // namespace
+
+extern "C" {
+
+pk_status pk_kernel_stream_attention(int device, int math, int n_streams, int n_active, const int32_t *act_stream, const int32_t *row_off,
+                                     int rows_total, const int32_t *cache_len, const int32_t *ring_start, int L, int d_model, int n_heads,
+                                     int tmax, const float *qkv, const float *pp, const float *pos_u, const float *pos_v, const float *kc,
+                                     const float *vc, float *ctx_f32, float *ctx_hi, float *ctx_lo, float *kc_out, float *vc_out,
+                                     int64_t *guard_bad) {
+    if (!streams_ok(n_streams, n_active, act_stream, row_off, rows_total) || !cache_len || !ring_start || L < 1 || n_heads < 1 ||
+        d_model % n_heads || !qkv || !pp || !pos_u || !pos_v || !kc || !vc || !kc_out || !vc_out || !act_out_ok(math, ctx_f32, ctx_hi, ctx_lo))
+        return PK_ERR_INVALID;
+    for (int s = 0; s < n_streams; ++s)
+        if (cache_len[s] < 0 || cache_len[s] > L || ring_start[s] < 0 || ring_start[s] >= L) return PK_ERR_INVALID;
+    const int maxC = max_len(row_off, n_active);
+    if (maxC < 1 || L + maxC > tmax) return PK_ERR_INVALID;
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const int d = d_model;
+    const size_t n_o = (size_t)rows_total * d, n_ring = (size_t)n_streams * L * d;
+    int32_t *dact = cx.upload(act_stream, n_active), *doff = cx.upload(row_off, n_active + 1);
+    int32_t *dcl = cx.upload(cache_len, n_streams), *drs = cx.upload(ring_start, n_streams);
+    float *dqkv = cx.upload(qkv, (size_t)rows_total * 3 * d), *dpp = cx.upload(pp, (size_t)(2 * tmax - 1) * d);
+    float *du = cx.upload(pos_u, d), *dv = cx.upload(pos_v, d);
+    float *dkc = guarded_state(cx, kc, n_ring), *dvc = guarded_state(cx, vc, n_ring);
+    ActBuf out = guarded_act(cx, math, n_o, ctx_lo != nullptr);
+    if (!cx.ok) return PK_ERR_CUDA;
+    if (!launch_stream_attention(dqkv, 3 * d, doff, dact, n_active, maxC, dcl, drs, dkc, dvc, L, n_heads, d / n_heads, d, dpp, tmax, du, dv,
+                                 out, cx.st))
+        return PK_ERR_INVALID;
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    if (!fetch_act(out, ctx_f32, ctx_hi, ctx_lo, n_o) || !fetch_f32(kc_out, dkc, n_ring) || !fetch_f32(vc_out, dvc, n_ring)) return PK_ERR_CUDA;
+    return PK_OK;
+}
+
+pk_status pk_kernel_stream_dwconv(int device, int math, int n_streams, int n_active, const int32_t *act_stream, const int32_t *row_off,
+                                  int rows_total, int d, int ks, const float *glu, const float *w, const float *bias, const float *cache,
+                                  float *out_f32, float *hi, float *lo, float *cache_out, int64_t *guard_bad) {
+    if (!streams_ok(n_streams, n_active, act_stream, row_off, rows_total) || d < 1 || ks < 2 || !glu || !w || !bias || !cache ||
+        !cache_out || !act_out_ok(math, out_f32, hi, lo))
+        return PK_ERR_INVALID;
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const size_t n_o = (size_t)rows_total * d, n_c = (size_t)n_streams * (ks - 1) * d;
+    int32_t *dact = cx.upload(act_stream, n_active), *doff = cx.upload(row_off, n_active + 1);
+    float *dg = cx.upload(glu, n_o), *dw = cx.upload(w, (size_t)d * ks), *db = cx.upload(bias, d);
+    float *dc = guarded_state(cx, cache, n_c);
+    ActBuf out = guarded_act(cx, math, n_o, lo != nullptr);
+    if (!cx.ok) return PK_ERR_CUDA;
+    if (!launch_stream_dwconv(dg, doff, dact, n_active, dc, d, ks, dw, db, out, cx.st)) return PK_ERR_INVALID;
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    if (!fetch_act(out, out_f32, hi, lo, n_o) || !fetch_f32(cache_out, dc, n_c)) return PK_ERR_CUDA;
+    return PK_OK;
+}
+
+}  // extern "C"

@@ -63,12 +63,13 @@ class TdtHookOut(C.Structure):
         [(n, C.c_int32) for n in ("steps", "grid", "cl", "upc", "opc", "out_in_smem", "wih_in_smem", "staged_ih", "wstage_rows")]
 
 
-EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_engine_create", "pk_engine_destroy", "pk_last_error",
+EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_config_nemotron_600m", "pk_engine_create", "pk_engine_destroy", "pk_last_error",
            "pk_mel_frames", "pk_encoder_frames", "pk_mel", "pk_encode", "pk_decode", "pk_ctc_logprobs",
            "pk_transcribe_batch", "pk_stage_pcm", "pk_prefetch_pcm", "pk_run_staged", "pk_fetch_tokens", "pk_sync",
            "pk_token_buffer", "pk_stream", "pk_launch_count", "pk_profile_begin", "pk_profile_end",
            "pk_profile_names", "pk_flush_l2", "pk_selftest_gemm", "pk_selftest_gemm_ln", "pk_selftest_attention",
-           "pk_kernel_gemm", "pk_kernel_attention", "pk_kernel_layernorm", "pk_kernel_dwconv", "pk_kernel_ctc_argmax", "pk_kernel_tdt_decode", "pk_debug_tdt_phases", "pk_vocab_load", "pk_vocab_free", "pk_vocab_size",
+           "pk_kernel_gemm", "pk_kernel_attention", "pk_kernel_layernorm", "pk_kernel_dwconv", "pk_kernel_ctc_argmax", "pk_kernel_tdt_decode", "pk_kernel_stream_attention", "pk_kernel_stream_dwconv",
+           "pk_debug_tdt_phases", "pk_vocab_load", "pk_vocab_free", "pk_vocab_size",
            "pk_detokenize", "pk_group_words", "pk_tokenize", "pk_ctc_decode_boosted",
            "pk_resample_len", "pk_resample",
            "pk_job_begin", "pk_job_append", "pk_nccl_unique_id", "pk_comm_init_rank", "pk_allgather_tokens",
@@ -93,6 +94,7 @@ def load_library():
     L.pk_config_110m.argtypes = [C.POINTER(_PkConfig)]
     L.pk_config_tdt_600m.argtypes = [C.POINTER(_PkConfig)]
     L.pk_config_rnnt_600m.argtypes = [C.POINTER(_PkConfig)]
+    L.pk_config_nemotron_600m.argtypes = [C.POINTER(_PkConfig)]
     L.pk_engine_create.argtypes = [C.POINTER(_PkConfig), C.c_char_p, C.c_int, C.POINTER(vp)]
     L.pk_engine_destroy.argtypes = [vp]
     L.pk_last_error.argtypes = [vp]
@@ -138,6 +140,8 @@ def load_library():
     L.pk_kernel_dwconv.argtypes = [C.c_int] * 3 + [i32p] + [C.c_int] * 3 + [f32p] * 6 + [i64p]
     L.pk_kernel_ctc_argmax.argtypes = [C.c_int] * 4 + [f32p, i32p, f32p, f32p, i64p]
     L.pk_kernel_tdt_decode.argtypes = [C.c_int, C.POINTER(TdtHookIn), C.POINTER(TdtHookOut), i64p]
+    L.pk_kernel_stream_attention.argtypes = [C.c_int] * 4 + [i32p, i32p, C.c_int, i32p, i32p] + [C.c_int] * 4 + [f32p] * 11 + [i64p]
+    L.pk_kernel_stream_dwconv.argtypes = [C.c_int] * 4 + [i32p, i32p] + [C.c_int] * 3 + [f32p] * 8 + [i64p]
     L.pk_vocab_load.argtypes = [C.c_char_p, C.POINTER(vp)]
     L.pk_vocab_free.argtypes = [vp]
     L.pk_vocab_size.argtypes = [vp]
@@ -239,6 +243,25 @@ def make_rnnt_600m_config(**kw) -> ModelConfig:      # config.hpp:118-135 (Parak
 def make_eou_120m_config(**kw) -> ModelConfig:       # eou.hpp:32-55 (streaming; ParakeetEOU registers "joint_", eou.cpp:9-13)
     base = dict(has_ctc=False, joint_prefix="joint_.", name="eou-120m", att_context_left=70, att_context_right=1,
                 max_batch=64, max_samples=102400)
+    base.update(kw)
+    return ModelConfig(**base)
+
+
+def make_nemotron_600m_config(latency_frames: int = 0, **kw) -> ModelConfig:   # nemotron.hpp:33-54
+    """The multilingual streaming model (ParakeetNemotron registers "encoder_" / "prediction_" / "joint_", the eou layout).
+    latency_frames is att_context_right; like the reference's CPU path, it does not change the output (DESIGN.md)."""
+    base = dict(d_model=1024, n_layers=24, ff=4096, vocab=8193, lstm_layers=2, has_ctc=False, joint_prefix="joint_.",
+                name="nemotron-600m", att_context_left=70, att_context_right=latency_frames, max_batch=64, max_samples=102400)
+    base.update(kw)
+    return ModelConfig(**base)
+
+
+def make_tiny_nemotron_config(**kw) -> ModelConfig:
+    """Small test-only streaming shape with the Nemotron preset's head_dim 128 and two LSTM layers
+    (mirrors tests/nemotron_oracle.make_tiny_nemotron_config; not a reference preset)."""
+    base = dict(sub_channels=64, d_model=256, n_layers=2, n_heads=2, ff=512, vocab=33, pred_hidden=64, lstm_layers=2,
+                joint_hidden=64, has_ctc=False, joint_prefix="joint_.", name="tiny-nemotron", att_context_left=12,
+                att_context_right=0, max_batch=8, max_samples=102400)
     base.update(kw)
     return ModelConfig(**base)
 
