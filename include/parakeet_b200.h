@@ -402,6 +402,48 @@ int32_t pk_ctc_decode_boosted(const float *logprobs, int32_t n_frames, int32_t v
  * PK_ERR_INVALID there (streaming decodes eou's TDT joint). */
 pk_status pk_set_boost(pk_engine *e, const int32_t *phrase_ids, const int32_t *phrase_off, int32_t n_phrases, float boost);
 
+/* Offline speaker diarization: Sortformer (include/parakeet/sortformer.hpp, src/sortformer.cpp:42-122 of the reference).
+ * PCM -> log-mel WITHOUT per-bin normalisation (main.cpp:514-517) -> NEST encoder (the offline FastConformer under keys
+ * "nest_encoder_.", subsampling output times sqrt(d_model), streaming_encoder.cpp:399-423) -> projection_ -> transformer_
+ * (post-norm blocks, head_dim 24, transformer.cpp:15-62) -> sigmoid(output_proj_(ReLU(first_hidden_(ReLU(.))))).
+ * enc: the NEST encoder's shape plus the engine capacity and math (decoder fields are ignored). */
+typedef struct {
+    pk_config enc;
+    int32_t t_hidden;       /* 192 */
+    int32_t t_layers;       /* 18 */
+    int32_t t_heads;        /* 8 (head_dim 24: the only one the attention kernel takes) */
+    int32_t t_ff;           /* 768 */
+    int32_t max_speakers;   /* 4 */
+} pk_sortformer_config;
+/* make_sortformer_117m_config (sortformer.hpp:43-72): NEST 17 x d 512, 8 heads, ff 2048, 128 mels, 256 subsampling channels;
+ * transformer 18 x d 192, 8 heads, ff 768; 4 speakers.  Capacity: 16 utterances of 90 s, bf16x3. */
+void pk_config_sortformer_117m(pk_sortformer_config *cfg);
+/* An engine in diarization mode.  Required keys: nest_encoder_.*, projection_, transformer_.layers_.{i}.{norm1_, mha_.{q,k,v,out}_proj,
+ * norm2_, fc1_, fc2_}, first_hidden_, output_proj_ (hidden_to_spks_ is not used and not required).  On it pk_mel, pk_encode
+ * (the NEST encoder output), pk_stage_pcm, the profile calls and pk_last_error work; the decode, boosting and streaming entry
+ * points return PK_ERR_INVALID. */
+pk_status pk_sortformer_create(const pk_sortformer_config *cfg, const char *safetensors_path, int device, pk_engine **out);
+/* Sortformer::forward on a batch of features (packed (sum frames_i, mel_bins), as pk_mel returns them): probs_out packed
+ * (sum T'_i, max_speakers) sigmoid activities, t_out[n_utt] = T'_i (may be NULL). */
+pk_status pk_sortformer_forward(pk_engine *e, const float *feats, const int32_t *n_frames, int32_t n_utt, float *probs_out, int32_t *t_out);
+/* The whole path from 16 kHz PCM (utterance i = pcm[offsets[i] .. offsets[i+1])); outputs as pk_sortformer_forward. */
+pk_status pk_diarize_batch(pk_engine *e, const float *pcm, const int64_t *offsets, int32_t n_utt, float *probs_out, int32_t *t_out);
+/* Device-resident form (measurement): pk_stage_pcm, then pk_run_diarize_staged (one CUDA graph per batch shape after the front
+ * end), then pk_fetch_probs. */
+pk_status pk_run_diarize_staged(pk_engine *e);
+pk_status pk_fetch_probs(pk_engine *e, float *probs_out, int32_t *t_out);
+/* Sortformer::probs_to_segments (sortformer.cpp:70-113) for one utterance, on the host: probs [T][S]; a frame is active when
+ * p > threshold; a segment is [start frame, last active frame] in seconds (frame * 0.08 s); segments sorted by start, equal
+ * starts by speaker id.  Writes at most cap segments; returns their full number, or -1 on invalid arguments. */
+int32_t pk_diar_segments(const float *probs, int32_t T, int32_t S, float threshold, int32_t *spk, float *start, float *end, int32_t cap);
+/* Kernel test hooks (conventions of the pk_kernel_* hooks above).  pk_kernel_mha: the transformer attention on qkv [rows_total][3 d]
+ * fp32 (q | k | v), head_dim 24 only (else PK_ERR_INVALID); ctx [rows_total][d] in ctx_f32 with PK_MATH_FP32, else ctx_hi and,
+ * with PK_MATH_BF16X3, ctx_lo.  pk_kernel_speaker_head: x [M][D], w1 [D][D], b1 [D], w2 [S][D], b2 [S] -> probs [M][S]. */
+pk_status pk_kernel_mha(int device, int math, int n_utt, const int32_t *row_off, int rows_total, int d_model, int n_heads, const float *qkv,
+                        float *ctx_f32, float *ctx_hi, float *ctx_lo, int64_t *guard_bad);
+pk_status pk_kernel_speaker_head(int device, int M, int D, int S, const float *x, const float *w1, const float *b1, const float *w2,
+                                 const float *b2, float *probs, int64_t *guard_bad);
+
 /* Sample-rate conversion (widening row: SURVEY.md section 8f(4)), replacing parakeet::resample / sinc_resample
  * (src/audio_io.cpp:123-195, :238-251): 32-tap Kaiser (beta 7.857) windowed sinc in double, output length
  * ceil(n * dst / src) (pk_resample_len), implemented as a POLYPHASE filter: the weights depend only on the phase

@@ -13,4 +13,5 @@ from .engine import (Decoder, Engine, ModelConfig, TranscribeOptions, Transcribe
                      TimestampedToken, WordTimestamp, lib_path, load_library, make_110m_config,
                      make_tdt_600m_config, make_tiny_config, make_eou_120m_config, make_tiny_stream_config,
                      make_rnnt_600m_config, make_tiny_rnnt_config, make_nemotron_600m_config,
-                     make_tiny_nemotron_config)
+                     make_tiny_nemotron_config, SortformerConfig, DiarizationSegment, diar_segments,
+                     make_sortformer_117m_config, make_tiny_sortformer_config)

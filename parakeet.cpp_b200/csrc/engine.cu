@@ -17,6 +17,8 @@
 // sequence end the batch-1 reference gives it.
 #include "engine.h"
 
+#include <algorithm>
+
 namespace pk_detail {
 std::string &create_err() {
     thread_local std::string s;
@@ -62,7 +64,7 @@ pk_status pk_engine::finish_weight(std::vector<float> &w, std::vector<float> *b,
 
 pk_status pk_engine::make_weight(const SafeTensors &st, const std::string &wname, const std::string &bname, int N,
                                  int K, GemmWeight &out, const std::vector<int> *row_perm,
-                                 const std::vector<int> *col_perm) {
+                                 const std::vector<int> *col_perm, float scale) {
     std::vector<float> w, b;
     std::string e;
     if (!st.read_f32(wname, w, (int64_t)N * K, e)) return fail(PK_ERR_MISSING, e);
@@ -79,6 +81,10 @@ pk_status pk_engine::make_weight(const SafeTensors &st, const std::string &wname
         }
         w.swap(w2);
         if (!b.empty()) b.swap(b2);
+    }
+    if (scale != 1.0f) {
+        for (auto &v : w) v *= scale;
+        for (auto &v : b) v *= scale;
     }
     return finish_weight(w, bname.empty() ? nullptr : &b, N, K, out);
 }
@@ -138,7 +144,7 @@ pk_status pk_engine::load(const char *path) {
     }
 
     // ---- subsampling (encoder.cpp:208-241)
-    const std::string sp = "encoder_.subsampling_.";
+    const std::string sp = enc_prefix + "subsampling_.";
     if ((s = get_vec(st, sp + "conv1_.weight", C * 9, &c1_w))) return s;
     if ((s = get_vec(st, sp + "conv1_.bias", C, &c1_b))) return s;
     if ((s = get_vec(st, sp + "dw1_.weight", C * 9, &dw1_w))) return s;
@@ -160,7 +166,11 @@ pk_status pk_engine::load(const char *path) {
         std::vector<int> colp((size_t)C * f3n);
         for (int f = 0; f < f3n; ++f)
             for (int ch = 0; ch < C; ++ch) colp[(size_t)f * C + ch] = ch * f3n + f;
-        if ((s = make_weight(st, sp + "proj_.weight", sp + "proj_.bias", d, C * f3n, proj, nullptr, &colp))) return s;
+        // xscaling (StreamingFastConformerEncoder::forward, streaming_encoder.cpp:403-407): the NEST encoder multiplies the
+        // subsampling output by sqrt(d) before layer 0.  Folded into proj_ here, before the hi/lo split: (s W) x + s b
+        // rounds differently from s (W x + b) by about one fp32 rounding.
+        const float xscale = diar ? std::sqrt((float)d) : 1.0f;
+        if ((s = make_weight(st, sp + "proj_.weight", sp + "proj_.bias", d, C * f3n, proj, nullptr, &colp, xscale))) return s;
     }
 
     // ---- relative position table input: emb(p) for p = -(Tmax-1) .. Tmax-1, fp32 math as
@@ -181,7 +191,7 @@ pk_status pk_engine::load(const char *path) {
     layers.resize(c.n_layers);
     for (int i = 0; i < c.n_layers; ++i) {
         LayerW &L = layers[i];
-        const std::string lp = "encoder_.layers_." + std::to_string(i) + ".";
+        const std::string lp = enc_prefix + "layers_." + std::to_string(i) + ".";
         for (int f = 0; f < 2; ++f) {
             const std::string fp = lp + (f == 0 ? "ffn1_." : "ffn2_.");
             if ((s = get_vec(st, fp + "norm_.weight", d, &L.ffn_ln_w[f]))) return s;
@@ -267,6 +277,46 @@ pk_status pk_engine::load(const char *path) {
         }
         if ((s = get_vec(st, lp + "final_norm_.weight", d, &L.fin_ln_w))) return s;
         if ((s = get_vec(st, lp + "final_norm_.bias", d, &L.fin_ln_b))) return s;
+    }
+
+    if (diar) {   // Sortformer (sortformer.cpp:42-48): projection_, transformer_, first_hidden_, output_proj_ (hidden_to_spks_ unused)
+        const int Dt = sf.t_hidden, S = sf.max_speakers;
+        if ((s = make_weight(st, "projection_.weight", "projection_.bias", Dt, d, t_proj))) return s;
+        tlayers.resize(sf.t_layers);
+        for (int i = 0; i < sf.t_layers; ++i) {
+            TLayerW &L = tlayers[i];
+            const std::string lp = "transformer_.layers_." + std::to_string(i) + ".";
+            std::vector<float> w((size_t)3 * Dt * Dt), b((size_t)3 * Dt), t;
+            const char *names[3] = {"q_proj", "k_proj", "v_proj"};
+            for (int q = 0; q < 3; ++q) {
+                if (!st.read_f32(lp + "mha_." + names[q] + ".weight", t, (int64_t)Dt * Dt, e)) return fail(PK_ERR_MISSING, e);
+                memcpy(&w[(size_t)q * Dt * Dt], t.data(), t.size() * 4);
+                if (!st.read_f32(lp + "mha_." + names[q] + ".bias", t, Dt, e)) return fail(PK_ERR_MISSING, e);
+                memcpy(&b[(size_t)q * Dt], t.data(), t.size() * 4);
+            }
+            if ((s = finish_weight(w, &b, 3 * Dt, Dt, L.qkv))) return s;
+            if ((s = make_weight(st, lp + "mha_.out_proj.weight", lp + "mha_.out_proj.bias", Dt, Dt, L.out))) return s;
+            if ((s = make_weight(st, lp + "fc1_.weight", lp + "fc1_.bias", sf.t_ff, Dt, L.fc1))) return s;
+            if ((s = make_weight(st, lp + "fc2_.weight", lp + "fc2_.bias", Dt, sf.t_ff, L.fc2))) return s;
+            if ((s = get_vec(st, lp + "norm1_.weight", Dt, &L.n1_w))) return s;
+            if ((s = get_vec(st, lp + "norm1_.bias", Dt, &L.n1_b))) return s;
+            if ((s = get_vec(st, lp + "norm2_.weight", Dt, &L.n2_w))) return s;
+            if ((s = get_vec(st, lp + "norm2_.bias", Dt, &L.n2_b))) return s;
+        }
+        {
+            std::vector<float> w1, w1t((size_t)Dt * Dt);
+            if (!st.read_f32("first_hidden_.weight", w1, (int64_t)Dt * Dt, e)) return fail(PK_ERR_MISSING, e);
+            for (int n = 0; n < Dt; ++n)
+                for (int k = 0; k < Dt; ++k) w1t[(size_t)k * Dt + n] = w1[(size_t)n * Dt + k];
+            head_w1t = upload(w1t);
+            if (!head_w1t) return fail(PK_ERR_CUDA, "cudaMalloc failed (speaker head)");
+        }
+        if ((s = get_vec(st, "first_hidden_.bias", Dt, &head_b1))) return s;
+        if ((s = get_vec(st, "output_proj_.weight", S * Dt, &head_w2))) return s;
+        if ((s = get_vec(st, "output_proj_.bias", S, &head_b2))) return s;
+        PK_CUDA(cudaStreamSynchronize(stream));
+        PK_CUDA(cudaGetLastError());
+        return PK_OK;
     }
 
     // ---- heads
@@ -403,6 +453,23 @@ pk_status pk_engine::alloc_workspace() {
     if (!pl_sum || !tdt_keys || !hbuf || !x || !sub2 || !d_pcm || !t_conf || !skinny_ws || !skinny_tickets || !mel_part) return fail(PK_ERR_CUDA, "cudaMalloc failed (workspace)");
     if (cfg.math != PK_MATH_FP32 && (!sub1.hi || !sub3.hi || !sub4.hi || !ln.hi || !ffh.hi || !ctx.hi || !cv.hi))
         return fail(PK_ERR_CUDA, "workspace: cudaMalloc or cuTensorMapEncodeTiled failed for an activation operand");
+    if (diar) {
+        const int Dt = sf.t_hidden;
+        t_x = dalloc<float>(Mx * Dt);
+        t_qkv = dalloc<float>(Mx * 3 * Dt);
+        if (cfg.math != PK_MATH_FP32) {
+            t_kv_hi = dalloc<bf16>(Mx * 2 * Dt);
+            if (cfg.math == PK_MATH_BF16X3) t_kv_lo = dalloc<bf16>(Mx * 2 * Dt);
+            if (!t_kv_hi || (cfg.math == PK_MATH_BF16X3 && !t_kv_lo)) return fail(PK_ERR_CUDA, "cudaMalloc failed (k | v planes)");
+        }
+        probs = dalloc<float>(Mx * sf.max_speakers);
+        t_ln = act_alloc(Mx, Dt);
+        t_ctx = act_alloc(Mx, Dt);
+        t_ff = act_alloc(Mx, sf.t_ff);
+        if (!t_x || !t_qkv || !probs || (cfg.math == PK_MATH_FP32 ? (!t_ln.f32 || !t_ctx.f32 || !t_ff.f32) : (!t_ln.hi || !t_ctx.hi || !t_ff.hi)))
+            return fail(PK_ERR_CUDA, "cudaMalloc or cuTensorMapEncodeTiled failed (transformer workspace)");
+        PK_CUDA(cudaMallocHost(&h_probs, Mx * sf.max_speakers * sizeof(float)));
+    }
     PK_CUDA(cudaMallocHost(&h_pcm, (B * (size_t)c.max_samples + 8) * sizeof(float)));
     PK_CUDA(cudaMallocHost(&h_meta, (size_t)(8 * (B + 1)) * sizeof(int32_t)));
     PK_CUDA(cudaMallocHost(&h_tok, B * (1 + (size_t)cap) * sizeof(int32_t)));
@@ -417,6 +484,7 @@ pk_status pk_engine::set_batch_shapes(const int32_t *n_frames, const int64_t *of
     if (n <= 0) return fail(PK_ERR_INVALID, "empty batch");
     if (n > Bmax) return fail(PK_ERR_CAPACITY, "batch of " + std::to_string(n) + " exceeds max_batch " + std::to_string(Bmax));
     n_utt = n;
+    probs_valid = false;
     pcm_off.assign(n + 1, 0);
     frame_off.assign(n + 1, 0);
     s2_off.assign(n + 1, 0);
@@ -495,8 +563,8 @@ pk_status pk_engine::run_mel(int u0, int u1) {
     if (u1 <= u0) return PK_OK;
     Scope sc(this, CAT_MEL);
     launch_mel(pcm_src ? pcm_src : d_pcm, d_pcm_off + u0, d_frame_off + u0, u1 - u0, maxF, cfg.mel_bins, mel_tb, logmel, feats,
-               mel_part + mel_part_floats(u0, cfg.mel_bins), stream);
-    launches += 3;
+               mel_part + mel_part_floats(u0, cfg.mel_bins), stream, !diar);
+    launches += diar ? 1 : 3;
     PK_CUDA(cudaGetLastError());
     return PK_OK;
 }
@@ -765,6 +833,80 @@ pk_status pk_engine::run_tdt() {
     return PK_OK;
 }
 
+// Sortformer::forward after the NEST encoder (sortformer.cpp:54-67; transformer.cpp:15-62 with pre_ln = false): projection_,
+// 18 post-norm blocks
+//     x = norm1_(x + out_proj(MHA(x)));   x = norm2_(x + fc2(ReLU(fc1(x))))
+// then the fused speaker head.  The fp32 residual stream is t_x; every LayerNorm also writes the next GEMM's operand.
+pk_status pk_engine::run_diar_head() {
+    const int Dt = sf.t_hidden, H = sf.t_heads;
+    const bool f32 = cfg.math == PK_MATH_FP32;
+    Act xo;                                   // t_x as a GEMM operand
+    if (f32) xo.f32 = t_x; else xo = t_ln;
+    ActBuf planes;                            // what a LayerNorm writes besides t_x
+    if (!f32) planes = t_ln;
+    {
+        EpiParams ep;
+        ep.kind = EPI_BIAS_F32;
+        ep.out_f32 = t_x;
+        ep.ldo = Dt;
+        gemm(enc_operand(this), cfg.d_model, t_proj, M, ep);
+        if (!f32) {
+            Scope sc(this, CAT_LAYERNORM);
+            launch_split(t_x, (size_t)M * Dt, t_ln, stream);
+            ++launches;
+        }
+    }
+    ActBuf none;
+    for (const TLayerW &L : tlayers) {
+        EpiParams eq;
+        if (f32) {           // q | k | v fp32 [M][3 d] for the CUDA-core attention
+            eq.kind = EPI_BIAS_F32;
+            eq.out_f32 = t_qkv;
+            eq.ldo = 3 * Dt;
+        } else {             // q fp32 [M][d], k | v bf16 planes [M][2 d] for the tensor-core attention
+            eq.kind = EPI_QKV_ACT;
+            eq.out_f32 = t_qkv;
+            eq.qcols = Dt;
+            eq.act.hi = t_kv_hi;
+            eq.act.lo = t_kv_lo;
+            eq.ldo = 2 * Dt;
+        }
+        gemm(xo, Dt, L.qkv, M, eq);
+        {
+            Scope sc(this, CAT_MHA);
+            const bool ok = f32 ? launch_mha_attention(t_qkv, 3 * Dt, d_row_off, n_utt, maxT, H, Dt / H, Dt, t_ctx, stream)
+                                : launch_mha_attention_tc(t_qkv, t_kv_hi, t_kv_lo, 2 * Dt, d_row_off, n_utt, maxT, H, Dt / H, Dt, t_ctx, stream);
+            if (!ok) return fail(PK_ERR_INVALID, "transformer attention: unsupported head_dim " + std::to_string(Dt / H));
+        }
+        ++launches;
+        EpiParams er;
+        er.kind = EPI_RESID_F32;
+        er.out_f32 = t_x;
+        er.resid = t_x;
+        er.ldo = Dt;
+        er.alpha = 1.0f;
+        gemm(t_ctx, Dt, L.out, M, er);
+        PK_LN(t_x, M, Dt, L.n1_w, L.n1_b, t_x, planes, nullptr, nullptr, none, stream);
+        ++launches;
+        EpiParams e1;
+        e1.kind = EPI_BIAS_RELU_ACT;
+        e1.act = t_ff;
+        e1.ldo = sf.t_ff;
+        gemm(xo, Dt, L.fc1, M, e1);
+        gemm(t_ff, sf.t_ff, L.fc2, M, er);
+        PK_LN(t_x, M, Dt, L.n2_w, L.n2_b, t_x, planes, nullptr, nullptr, none, stream);
+        ++launches;
+    }
+    {
+        Scope sc(this, CAT_HEAD);
+        if (!launch_speaker_head(t_x, M, Dt, sf.max_speakers, head_w1t, head_b1, head_w2, head_b2, probs, num_sms, stream))
+            return fail(PK_ERR_INVALID, "speaker head: unsupported shape");
+    }
+    ++launches;
+    PK_CUDA(cudaGetLastError());
+    return PK_OK;
+}
+
 pk_status pk_engine::fetch(pk_tokens *out) {
     if (!out || !out->ids || !out->len) return fail(PK_ERR_INVALID, "pk_tokens needs ids and len");
     const size_t n = n_utt;
@@ -880,6 +1022,8 @@ int32_t pk_encoder_frames(int32_t f) { return conv_len(conv_len(conv_len(f))); }
 
 const char *pk_last_error(const pk_engine *e) { return e ? e->err.c_str() : g_create_err.c_str(); }
 
+static pk_status create_engine(const pk_config &c, const pk_sortformer_config *sf, const char *path, int device, pk_engine **out);
+
 pk_status pk_engine_create(const pk_config *cfg, const char *path, int device, pk_engine **out) {
     if (!cfg || !path || !out) {
         g_create_err = "null argument";
@@ -915,8 +1059,20 @@ pk_status pk_engine_create(const pk_config *cfg, const char *path, int device, p
         g_create_err = "unknown pk_math mode";
         return PK_ERR_INVALID;
     }
+    return create_engine(c, nullptr, path, device, out);
+}
+
+// Everything of engine creation after the config checks; sf != NULL: a Sortformer engine (pk_sortformer_create).
+static pk_status create_engine(const pk_config &c, const pk_sortformer_config *sf, const char *path, int device, pk_engine **out) {
     auto e = std::make_unique<pk_engine>();
     e->cfg = c;
+    if (sf) {
+        e->diar = true;
+        e->sf = *sf;
+        e->enc_prefix = "nest_encoder_.";
+        // every row through the same GEMM kernel whatever the batch: an utterance's activities do not depend on its batch
+        e->skinny = false;
+    }
     if (const char *ev = getenv("PK_GRAPH")) e->use_graphs = atoi(ev) != 0;
     if (const char *ev = getenv("PK_ATTN_TC")) e->attn_tc = atoi(ev) != 0;
     if (const char *ev = getenv("PK_ATTN_UMMA")) e->attn_wgmma = atoi(ev) != 0;
@@ -986,6 +1142,7 @@ void pk_engine_destroy(pk_engine *e) {
     if (e->h_ts) cudaFreeHost(e->h_ts);
     if (e->h_te) cudaFreeHost(e->h_te);
     if (e->h_tc) cudaFreeHost(e->h_tc);
+    if (e->h_probs) cudaFreeHost(e->h_probs);
     if (e->ev_h2d) cudaEventDestroy(e->ev_h2d);
     if (e->ev_front) cudaEventDestroy(e->ev_front);
     for (int i = 0; i < pk_engine::H2D_CHUNKS; ++i)
@@ -1008,15 +1165,18 @@ pk_status pk_profile_begin(pk_engine *e) {
 }
 
 pk_status pk_profile_end(pk_engine *e, double *ms, int64_t *counts, double *flops, int32_t n) {
-    if (!e || !ms || !counts || n < pk_engine::CAT_N) return PK_ERR_INVALID;
+    // n >= 8: callers sized for the eight ASR classes (mel .. tdt) still get those; the diarization classes follow them
+    if (!e || !ms || !counts || n < pk_engine::CAT_MHA) return PK_ERR_INVALID;
     cudaStreamSynchronize(e->stream);
     for (int i = 0; i < n; ++i) { ms[i] = 0; counts[i] = 0; if (flops) flops[i] = 0; }
     for (auto &r : e->prof) {
         float t = 0.f;
         cudaEventElapsedTime(&t, r.a, r.b);
-        ms[r.cat] += t;
-        counts[r.cat] += 1;
-        if (flops) flops[r.cat] += r.flops;
+        if (r.cat < n) {
+            ms[r.cat] += t;
+            counts[r.cat] += 1;
+            if (flops) flops[r.cat] += r.flops;
+        }
         e->ev_pool.push_back(r.a);
         e->ev_pool.push_back(r.b);
     }
@@ -1025,7 +1185,7 @@ pk_status pk_profile_end(pk_engine *e, double *ms, int64_t *counts, double *flop
     return PK_OK;
 }
 
-const char *pk_profile_names(void) { return "mel,subsample,gemm,layernorm,attention,dwconv,ctc,tdt"; }
+const char *pk_profile_names(void) { return "mel,subsample,gemm,layernorm,attention,dwconv,ctc,tdt,mha,speaker_head"; }
 
 pk_status pk_flush_l2(pk_engine *e) {
     if (!e) return PK_ERR_INVALID;
@@ -1523,6 +1683,7 @@ static pk_status run_front(pk_engine *e) {
 // TDT and RNN-T share the decode kernel but not the joint: each decoder runs only on its own model
 // (a model without a CTC head rejects PK_DECODER_CTC in run_ctc).
 static pk_status check_decoder(pk_engine *e, pk_decoder dec) {
+    if (e->diar) return e->fail(PK_ERR_INVALID, "a Sortformer engine has no decoder: use pk_sortformer_forward / pk_diarize_batch");
     const bool rnnt_model = e->cfg.n_durations == 0;
     if (dec == PK_DECODER_TDT && rnnt_model)
         return e->fail(PK_ERR_INVALID, "PK_DECODER_TDT on an RNN-T model (n_durations = 0): use PK_DECODER_RNNT");
@@ -1557,6 +1718,7 @@ pk_status pk_run_staged(pk_engine *e, pk_decoder dec) {
 
 pk_status pk_fetch_tokens(pk_engine *e, pk_tokens *out) {
     if (!e) return PK_ERR_INVALID;
+    if (e->diar) return e->fail(PK_ERR_INVALID, "a Sortformer engine has no decoder: use pk_fetch_probs");
     cudaSetDevice(e->device);
     return e->fetch(out);
 }
@@ -1811,6 +1973,7 @@ pk_status pk_resample_batch(pk_engine *e, const float *pcm, const int64_t *offse
 // sorted by token) and uploaded; the decode kernels (ctc.cu: ctc_boosted_decode_kernel, tdt.cu: boost_on) walk it.
 pk_status pk_set_boost(pk_engine *e, const int32_t *phrase_ids, const int32_t *phrase_off, int32_t n_phrases, float boost) {
     if (!e || n_phrases < 0 || (n_phrases > 0 && (!phrase_ids || !phrase_off))) return PK_ERR_INVALID;
+    if (e->diar) return e->fail(PK_ERR_INVALID, "pk_set_boost: a Sortformer engine has no decoder");
     if (e->cfg.n_durations == 0 && n_phrases > 0)
         return e->fail(PK_ERR_INVALID, "pk_set_boost: phrase boosting covers CTC and TDT decodes; this is an RNN-T model");
     cudaSetDevice(e->device);
@@ -1958,6 +2121,7 @@ pk_status pk_decode(pk_engine *e, const float *enc, const int32_t *enc_lens, int
 
 pk_status pk_ctc_logprobs(pk_engine *e, const float *enc, int32_t total_frames, float *logprobs_out) {
     if (!e || !enc || !logprobs_out || total_frames < 1) return PK_ERR_INVALID;
+    if (e->diar) return e->fail(PK_ERR_INVALID, "a Sortformer engine has no CTC head");
     cudaSetDevice(e->device);
     if (total_frames > e->Tmax) return e->fail(PK_ERR_CAPACITY, "pk_ctc_logprobs: more than Tmax frames");
     pk_status s;
@@ -1971,6 +2135,151 @@ pk_status pk_ctc_logprobs(pk_engine *e, const float *enc, int32_t total_frames, 
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
     if (ce != cudaSuccess) return e->fail(PK_ERR_CUDA, std::string("pk_ctc_logprobs: ") + cudaGetErrorString(ce));
     return PK_OK;
+}
+
+// ===================================================================== Sortformer diarization (sortformer.cpp:42-122)
+
+void pk_config_sortformer_117m(pk_sortformer_config *c) {   // make_sortformer_117m_config, sortformer.hpp:43-72
+    memset(c, 0, sizeof(*c));
+    pk_config &e = c->enc;
+    e.mel_bins = 128; e.sub_channels = 256; e.d_model = 512; e.n_layers = 17; e.n_heads = 8; e.ff = 2048; e.conv_kernel = 9;
+    e.max_batch = 16; e.max_samples = 1440000; e.math = PK_MATH_BF16X3;
+    c->t_hidden = 192; c->t_layers = 18; c->t_heads = 8; c->t_ff = 768; c->max_speakers = 4;
+}
+
+pk_status pk_sortformer_create(const pk_sortformer_config *sf, const char *path, int device, pk_engine **out) {
+    if (!sf || !path || !out) {
+        g_create_err = "null argument";
+        return PK_ERR_INVALID;
+    }
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+        g_create_err = "no CUDA device: this engine has no CPU fallback";
+        return PK_ERR_CUDA;
+    }
+    if (device < 0 || device >= ndev) {
+        g_create_err = "bad device index";
+        return PK_ERR_INVALID;
+    }
+    const pk_config &c = sf->enc;
+    if (c.d_model % 128 || c.d_model % c.n_heads || c.mel_bins % 8 || c.sub_channels % 4 || c.ff % 16 || c.conv_kernel != 9 ||
+        c.max_batch < 1 || c.max_samples < 400 || c.sub_channels > 1024) {
+        g_create_err = "unsupported NEST encoder shape in pk_sortformer_config.enc";
+        return PK_ERR_INVALID;
+    }
+    if (c.math != PK_MATH_FP32 && c.math != PK_MATH_BF16X3 && c.math != PK_MATH_BF16X1) {
+        g_create_err = "unknown pk_math mode";
+        return PK_ERR_INVALID;
+    }
+    // The transformer's GEMMs take K = t_hidden and t_ff (K % 64 for the wgmma path), the attention kernel head_dim 24, the
+    // speaker head t_hidden % 32 <= 256.
+    if (sf->t_layers < 1 || sf->t_heads < 1 || sf->t_hidden != 24 * sf->t_heads || sf->t_hidden % 64 || sf->t_hidden > 256 ||
+        sf->t_ff < 64 || sf->t_ff % 64 || sf->max_speakers < 1 || sf->max_speakers > 64) {
+        g_create_err = "unsupported Sortformer transformer shape: needs head_dim 24, t_hidden a multiple of 64 up to 256, t_ff a multiple of 64";
+        return PK_ERR_INVALID;
+    }
+    if (speaker_head_smem(sf->t_hidden, sf->max_speakers) > 227 * 1024) {
+        g_create_err = "unsupported Sortformer speaker head: its weights do not fit in shared memory (t_hidden, max_speakers)";
+        return PK_ERR_INVALID;
+    }
+    pk_config cc = c;       // no decoder: its fields are not read
+    cc.vocab = 0; cc.pred_hidden = 0; cc.lstm_layers = 0; cc.joint_hidden = 0; cc.n_durations = 0; cc.has_ctc = 0; cc.max_symbols = 0;
+    memset(cc.durations, 0, sizeof(cc.durations));
+    return create_engine(cc, sf, path, device, out);
+}
+
+#define PK_ECUDA(expr)                                                                              \
+    do {                                                                                            \
+        cudaError_t _e = (expr);                                                                    \
+        if (_e != cudaSuccess) return e->fail(PK_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e)); \
+    } while (0)
+
+static pk_status check_diar(pk_engine *e) {
+    if (!e->diar) return e->fail(PK_ERR_INVALID, "not a Sortformer engine (pk_sortformer_create)");
+    return e->gemm_err;
+}
+
+pk_status pk_fetch_probs(pk_engine *e, float *probs_out, int32_t *t_out) {
+    if (!e || !probs_out) return PK_ERR_INVALID;
+    cudaSetDevice(e->device);
+    if (pk_status s = check_diar(e)) return s;
+    if (!e->probs_valid) return e->fail(PK_ERR_INVALID, "pk_fetch_probs: no diarization run since the batch was staged");
+    const size_t n = (size_t)e->M * e->sf.max_speakers;
+    PK_ECUDA(cudaMemcpyAsync(e->h_probs, e->probs, n * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+    PK_ECUDA(cudaStreamSynchronize(e->stream));
+    memcpy(probs_out, e->h_probs, n * sizeof(float));
+    if (t_out)
+        for (int i = 0; i < e->n_utt; ++i) t_out[i] = e->row_off[i + 1] - e->row_off[i];
+    return PK_OK;
+}
+
+pk_status pk_sortformer_forward(pk_engine *e, const float *feats, const int32_t *n_frames, int32_t n_utt, float *probs_out, int32_t *t_out) {
+    if (!e || !feats || !n_frames || !probs_out) return PK_ERR_INVALID;
+    cudaSetDevice(e->device);
+    pk_status s;
+    if ((s = check_diar(e))) return s;
+    if ((s = e->set_batch_shapes(n_frames, nullptr, n_utt))) return s;
+    if ((s = e->upload_shapes())) return s;
+    const size_t nf = (size_t)e->frame_off[n_utt] * e->cfg.mel_bins;
+    PK_ECUDA(cudaMemcpyAsync(e->feats, feats, nf * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+    if ((s = e->run_conv1())) return s;
+    if ((s = e->run_encoder(nullptr, nullptr))) return s;
+    if ((s = e->run_diar_head())) return s;
+    e->probs_valid = true;
+    return pk_fetch_probs(e, probs_out, t_out);
+}
+
+// After pk_stage_pcm: the whole model after the front end replays as one CUDA graph per batch shape.
+pk_status pk_run_diarize_staged(pk_engine *e) {
+    if (!e || e->n_utt <= 0) return PK_ERR_INVALID;
+    cudaSetDevice(e->device);
+    if (pk_status s = check_diar(e)) return s;
+    {
+        pk_status fs = run_front(e);
+        e->front_done = false;
+        if (fs) return fs;
+    }
+    std::string key(1, 'd');
+    key.append(reinterpret_cast<const char *>(e->frame_off.data()), e->frame_off.size() * sizeof(int32_t));
+    pk_status s = e->run_graphed(key, [e]() {
+        pk_status s = e->run_encoder(nullptr, nullptr);
+        return s ? s : e->run_diar_head();
+    });
+    e->probs_valid = s == PK_OK;
+    return s;
+}
+
+pk_status pk_diarize_batch(pk_engine *e, const float *pcm, const int64_t *offsets, int32_t n_utt, float *probs_out, int32_t *t_out) {
+    if (!e || !probs_out) return PK_ERR_INVALID;
+    pk_status s;
+    if ((s = check_diar(e))) return s;
+    if ((s = pk_stage_pcm(e, pcm, offsets, n_utt))) return s;
+    if ((s = pk_run_diarize_staged(e))) return s;
+    return pk_fetch_probs(e, probs_out, t_out);
+}
+
+// Sortformer::probs_to_segments (sortformer.cpp:70-113) on the host.
+int32_t pk_diar_segments(const float *probs, int32_t T, int32_t S, float threshold, int32_t *spk, float *start, float *end, int32_t cap) {
+    if (!probs || T < 0 || S < 1 || cap < 0 || (cap > 0 && (!spk || !start || !end))) return -1;
+    struct Seg { int32_t s, t0, t1; };
+    std::vector<Seg> segs;
+    for (int s = 0; s < S; ++s) {
+        int t0 = -1;
+        for (int t = 0; t < T; ++t) {
+            const bool active = probs[(size_t)t * S + s] > threshold;   // strictly above
+            if (active && t0 < 0) t0 = t;
+            else if (!active && t0 >= 0) { segs.push_back({s, t0, t - 1}); t0 = -1; }
+        }
+        if (t0 >= 0) segs.push_back({s, t0, T - 1});
+    }
+    // by start; equal starts keep speaker order (what the reference's std::sort gives for <= 16 segments, DESIGN.md section 5)
+    std::stable_sort(segs.begin(), segs.end(), [](const Seg &a, const Seg &b) { return a.t0 < b.t0; });
+    for (size_t i = 0; i < segs.size() && (int64_t)i < cap; ++i) {
+        spk[i] = segs[i].s;
+        start[i] = (float)segs[i].t0 * 0.08f;   // frame_to_seconds, timestamp.hpp:31-35
+        end[i] = (float)segs[i].t1 * 0.08f;
+    }
+    return (int32_t)segs.size();
 }
 
 }  // extern "C"

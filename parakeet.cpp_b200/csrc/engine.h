@@ -66,11 +66,31 @@ struct LayerW {
     float *fin_ln_w, *fin_ln_b;
 };
 
+// One post-norm block of Sortformer's transformer_ (transformer.cpp:15-62).
+struct TLayerW {
+    GemmWeight qkv, out, fc1, fc2;   // q/k/v fused [3 d][d]
+    float *n1_w, *n1_b, *n2_w, *n2_b;
+};
+
 }  // namespace pk_detail
 using namespace pk_detail;
 
 struct pk_engine {
     pk_config cfg;
+    // ---- diarization mode (pk_sortformer_create): the NEST encoder is cfg's encoder under keys "nest_encoder_.", its
+    // subsampling output scaled by sqrt(d) (xscaling, folded into proj_), features not normalised; no decoder.
+    bool diar = false;
+    pk_sortformer_config sf{};
+    std::string enc_prefix = "encoder_.";
+    GemmWeight t_proj;                         // projection_ [t_hidden][d]
+    std::vector<TLayerW> tlayers;
+    float *head_w1t = nullptr, *head_b1 = nullptr, *head_w2 = nullptr, *head_b2 = nullptr;   // first_hidden_ (transposed), output_proj_
+    float *t_x = nullptr, *t_qkv = nullptr, *probs = nullptr;   // [Mx][t_hidden] residual stream, [Mx][3 t_hidden], [Mx][S]
+    Act t_ln, t_ctx, t_ff;                     // GEMM operands: LayerNorm output, attention context, ReLU(fc1)
+    bf16 *t_kv_hi = nullptr, *t_kv_lo = nullptr;   // [Mx][2 t_hidden] k | v planes of the tensor-core attention (q in t_qkv)
+    bool probs_valid = false;                  // probs hold the run of the staged batch
+    float *h_probs = nullptr;                  // pinned [Mx][S]
+    pk_status run_diar_head();                 // projection_ .. sigmoid on the encoder output in x
     int device = 0;
     int num_sms = 0;
     cudaStream_t stream = nullptr;
@@ -177,7 +197,7 @@ struct pk_engine {
     int32_t *trie_active = nullptr, *trie_nact = nullptr;
 
     // ---- optional per-kernel-class timing (CUDA events on the engine stream)
-    enum { CAT_MEL, CAT_SUBSAMPLE, CAT_GEMM, CAT_LAYERNORM, CAT_ATTENTION, CAT_DWCONV, CAT_CTC, CAT_TDT, CAT_N };
+    enum { CAT_MEL, CAT_SUBSAMPLE, CAT_GEMM, CAT_LAYERNORM, CAT_ATTENTION, CAT_DWCONV, CAT_CTC, CAT_TDT, CAT_MHA, CAT_HEAD, CAT_N };
     struct ProfRec { int cat; cudaEvent_t a, b; double flops; };
     bool prof_on = false;
     std::vector<ProfRec> prof;
@@ -237,7 +257,7 @@ struct pk_engine {
     pk_status load(const char *path);
     pk_status make_weight(const SafeTensors &st, const std::string &wname, const std::string &bname, int N, int K,
                           GemmWeight &out, const std::vector<int> *row_perm = nullptr,
-                          const std::vector<int> *col_perm = nullptr);
+                          const std::vector<int> *col_perm = nullptr, float scale = 1.0f);
     pk_status finish_weight(std::vector<float> &w, std::vector<float> *b, int N, int K, GemmWeight &out);
     pk_status get_vec(const SafeTensors &st, const std::string &name, int n, float **out);
     pk_status alloc_workspace();

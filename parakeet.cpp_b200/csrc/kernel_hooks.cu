@@ -253,7 +253,7 @@ pk_status pk_kernel_attention(int device, int kernel, int math, int n_utt, const
 
 pk_status pk_kernel_layernorm(int device, int M, int d, const float *x, const float *w1, const float *b1, const float *w2, const float *b2,
                               int want_f32, int planes, float *y1_f32, float *act_f32, float *hi, float *lo, int64_t *guard_bad) {
-    if (M < 1 || d < 128 || d > 1024 || d % 128 || !x || !w1 || !b1 || (!w2) != (!b2) || planes < 0 || planes > 3) return PK_ERR_INVALID;
+    if (M < 1 || d < 4 || d > 1024 || d % 4 || !x || !w1 || !b1 || (!w2) != (!b2) || planes < 0 || planes > 3) return PK_ERR_INVALID;
     if ((want_f32 && !y1_f32) || (planes == 3 && !act_f32) || ((planes == 1 || planes == 2) && !hi) || (planes == 2 && !lo)) return PK_ERR_INVALID;
     if (w2 && (!want_f32 || planes == 0)) return PK_ERR_INVALID;    // the chained form: y1 in place, LN2(y1) as the operand
     HookCtx cx(device);
@@ -578,6 +578,72 @@ pk_status pk_kernel_stream_dwconv(int device, int math, int n_streams, int n_act
     if (rc) return rc;
     if (!fetch_act(out, out_f32, hi, lo, n_o) || !fetch_f32(cache_out, dc, n_c)) return PK_ERR_CUDA;
     return PK_OK;
+}
+
+// Sortformer's transformer attention (attention_mha.cu) as the engine runs it in `math`: the fp32 kernel with PK_MATH_FP32,
+// else the mma.sync kernel on q fp32 and k | v split into bf16 planes.  qkv [rows_total][3 d] fp32; ctx [rows_total][d] as
+// the engine's transformer context buffer holds it (fp32 with PK_MATH_FP32, else bf16 hi | lo planes).
+pk_status pk_kernel_mha(int device, int math, int n_utt, const int32_t *row_off, int rows_total, int d_model, int n_heads, const float *qkv,
+                        float *ctx_f32, float *ctx_hi, float *ctx_lo, int64_t *guard_bad) {
+    if (!offsets_ok(row_off, n_utt, rows_total) || n_heads < 1 || d_model % n_heads || !qkv) return PK_ERR_INVALID;
+    const bool f32 = math == PK_MATH_FP32;
+    if (f32 ? !ctx_f32 : (!ctx_hi || (math == PK_MATH_BF16X3) != (ctx_lo != nullptr))) return PK_ERR_INVALID;
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const int d = d_model;
+    const size_t n_o = (size_t)rows_total * d;
+    int32_t *doff = cx.upload(row_off, n_utt + 1);
+    float *dqkv = cx.upload(qkv, (size_t)rows_total * 3 * d);
+    ActBuf out;
+    out.f32 = f32 ? cx.guarded<float>(n_o) : nullptr;
+    out.hi = f32 ? nullptr : cx.guarded<bf16>(n_o);
+    out.lo = ctx_lo ? cx.guarded<bf16>(n_o) : nullptr;
+    if (!cx.ok) return PK_ERR_CUDA;
+    bool launched;
+    if (f32) {
+        launched = launch_mha_attention(dqkv, 3 * d, doff, n_utt, max_len(row_off, n_utt), n_heads, d / n_heads, d, out, cx.st);
+    } else {
+        // the EPI_QKV_ACT epilogue's layout: q fp32 [M, d], k | v bf16 planes [M, 2 d]
+        std::vector<float> hq((size_t)rows_total * d), hkv((size_t)rows_total * 2 * d);
+        for (int r = 0; r < rows_total; ++r) {
+            memcpy(&hq[(size_t)r * d], qkv + (size_t)r * 3 * d, (size_t)d * 4);
+            memcpy(&hkv[(size_t)r * 2 * d], qkv + (size_t)r * 3 * d + d, (size_t)2 * d * 4);
+        }
+        float *dq32 = cx.upload(hq.data(), hq.size()), *dkv = cx.upload(hkv.data(), hkv.size());
+        ActBuf skv;
+        skv.hi = static_cast<bf16 *>(cx.alloc(hkv.size() * 2));
+        skv.lo = math == PK_MATH_BF16X3 ? static_cast<bf16 *>(cx.alloc(hkv.size() * 2)) : nullptr;
+        if (!cx.ok) return PK_ERR_CUDA;
+        launch_split(dkv, hkv.size(), skv, cx.st);
+        launched = launch_mha_attention_tc(dq32, skv.hi, skv.lo, 2 * d, doff, n_utt, max_len(row_off, n_utt), n_heads, d / n_heads, d, out, cx.st);
+    }
+    if (!launched) return PK_ERR_INVALID;
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    if (!fetch_f32(ctx_f32, out.f32, n_o) || (out.hi && !fetch_bf16(ctx_hi, out.hi, n_o)) || (out.lo && !fetch_bf16(ctx_lo, out.lo, n_o)))
+        return PK_ERR_CUDA;
+    return PK_OK;
+}
+
+// Sortformer's fused speaker head (speaker_head.cu): x [M][D], w1 [D][D] (first_hidden_, as stored), w2 [S][D] -> probs [M][S].
+pk_status pk_kernel_speaker_head(int device, int M, int D, int S, const float *x, const float *w1, const float *b1, const float *w2,
+                                 const float *b2, float *probs, int64_t *guard_bad) {
+    if (M < 1 || D < 1 || S < 1 || !x || !w1 || !b1 || !w2 || !b2 || !probs) return PK_ERR_INVALID;
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    std::vector<float> w1t((size_t)D * D);
+    for (int n = 0; n < D; ++n)
+        for (int k = 0; k < D; ++k) w1t[(size_t)k * D + n] = w1[(size_t)n * D + k];
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    float *dx = cx.upload(x, (size_t)M * D), *dw1 = cx.upload(w1t.data(), w1t.size()), *db1 = cx.upload(b1, D);
+    float *dw2 = cx.upload(w2, (size_t)S * D), *db2 = cx.upload(b2, S);
+    float *dp = cx.guarded<float>((size_t)M * S);
+    if (!cx.ok) return PK_ERR_CUDA;
+    if (!launch_speaker_head(dx, M, D, S, dw1, db1, dw2, db2, dp, sms, cx.st)) return PK_ERR_INVALID;
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    return fetch_f32(probs, dp, (size_t)M * S) ? PK_OK : PK_ERR_CUDA;
 }
 
 }  // extern "C"

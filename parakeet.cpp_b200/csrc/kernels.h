@@ -20,8 +20,10 @@ struct MelTables {
 size_t mel_smem_bytes(const MelTables &tb);
 // part: scratch of mel_part_floats(n_utt, n_mels) floats (per-chunk statistics of the normalisation), one slice per utterance
 size_t mel_part_floats(int n_utt, int n_mels);
+// normalize = false (Sortformer: preprocess_audio with AudioConfig::normalize off, main.cpp:514-517): K1 only, the
+// log-mel lands in feats and logmel / part are not used.
 void launch_mel(const float *pcm, const int64_t *pcm_off, const int32_t *frame_off, int n_utt, int max_frames,
-                int n_mels, const MelTables &tb, float *logmel, float *feats, float *part, cudaStream_t st);
+                int n_mels, const MelTables &tb, float *logmel, float *feats, float *part, cudaStream_t st, bool normalize = true);
 
 // streaming variant (StreamingAudioPreprocessor::process_chunk, src/audio.cpp:195-259): `sig` holds, per stream, the
 // already pre-emphasised samples [overlap | chunk]; frame f = window . sig[f*160 .. f*160+512) (center = False, no
@@ -140,6 +142,21 @@ bool relpos_attention_wgmma_supported(int head_dim, int max_T);
 bool launch_relpos_attention_wgmma(const float *q32, const float *pos_u, const float *pos_v, const bf16 *kv_hi, const bf16 *kv_lo, int ld_kv,
                                    const int32_t *row_off, int n_utt, int max_T, int n_heads, int head_dim, const bf16 *pp_hi, const bf16 *pp_lo,
                                    int tmax, int d_model, ActBuf out, cudaStream_t st);
+
+// ------------------------------------------------------------------ attention_mha.cu / speaker_head.cu (Sortformer)
+// Plain multi-head attention (transformer.cpp:15-50) over packed utterances, head_dim 24 only (false otherwise): qkv fp32
+// [M][ld_qkv] = q | k | v, out ctx [M][d_model].
+bool launch_mha_attention(const float *qkv, int ld_qkv, const int32_t *row_off, int n_utt, int max_T, int n_heads, int head_dim,
+                          int d_model, ActBuf out, cudaStream_t st);
+// Tensor-core form (bf16x3 with kv_lo, bf16x1 without): q32 fp32 [M][d_model], kv_hi / kv_lo = k | v bf16 planes [M][ld_kv] as
+// the EPI_QKV_ACT epilogue writes them.  head_dim 24 only (false otherwise).
+bool launch_mha_attention_tc(const float *q32, const bf16 *kv_hi, const bf16 *kv_lo, int ld_kv, const int32_t *row_off, int n_utt, int max_T,
+                             int n_heads, int head_dim, int d_model, ActBuf out, cudaStream_t st);
+// probs [M][S] = sigmoid(W2 . ReLU(W1 . ReLU(x) + b1) + b2) (sortformer.cpp:59-67); w1t = W1 transposed [D][D], w2 [S][D].
+// D % 32 == 0, D <= 256, S <= 64 (false otherwise).
+size_t speaker_head_smem(int D, int S);
+bool launch_speaker_head(const float *x, int M, int D, int S, const float *w1t, const float *b1, const float *w2, const float *b2,
+                         float *probs, int num_sms, cudaStream_t st);
 
 // ContextTrie (src/phrase_boost.cpp:9-66) in CSR form on the device: node 0 = root; the edges of node i are
 // [first[i], first[i+1]) = (token, child node), sorted by token.

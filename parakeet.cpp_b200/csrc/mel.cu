@@ -283,10 +283,11 @@ size_t mel_part_floats(int n_utt, int n_mels) { return (size_t)n_utt * MEL_CH * 
 
 void launch_mel(const float *pcm, const int64_t *pcm_off, const int32_t *frame_off, int n_utt,
                 int max_frames, int n_mels, const MelTables &tb, float *logmel, float *feats, float *part,
-                cudaStream_t st) {
+                cudaStream_t st, bool normalize) {
     dim3 grid((max_frames + WARPS * 4 - 1) / (WARPS * 4), n_utt);
     launch_pdl(mel_logpower_kernel<false>, dim3(grid), dim3(WARPS * 32), mel_smem_bytes(tb), st, pcm, pcm_off, frame_off, nullptr, n_mels, tb,
-                                                                             logmel);
+                                                                             normalize ? logmel : feats);
+    if (!normalize) return;
     int groups = 640 / n_mels;  // 8 for 80 bins, 5 for 128
     launch_pdl(mel_stats_kernel, dim3(MEL_CH, n_utt), dim3(groups * n_mels), sizeof(float) * groups * n_mels, st, logmel, frame_off, n_mels, part);
     launch_pdl(mel_apply_kernel, dim3(MEL_CH, n_utt), dim3(groups * n_mels), 0, st, logmel, frame_off, n_mels, part, feats);

@@ -17,16 +17,21 @@ namespace {
 
 constexpr int LN_MAXV = 8;  // float4 per lane: supports d <= 1024
 
+// Lane `lane` holds float4 number lane + 32 i of the row for i < nv; when d is not a multiple of 128 (Sortformer's d 192:
+// 48 float4), the last one exists only on the lanes with lane + 32 i < d / 4.
+__device__ __forceinline__ bool ln_has(int i, int nv, int lane, int d) { return i < nv && lane + 32 * i < (d >> 2); }
+
 __device__ __forceinline__ void ln_stats(const float4 *v, int nv, int d, float &mean, float &rstd, float eps) {
+    const int lane = threadIdx.x & 31;
     float s = 0.f;
 #pragma unroll
     for (int i = 0; i < LN_MAXV; ++i)
-        if (i < nv) s += v[i].x + v[i].y + v[i].z + v[i].w;
+        if (ln_has(i, nv, lane, d)) s += v[i].x + v[i].y + v[i].z + v[i].w;
     mean = warp_sum(s) / (float)d;
     float q = 0.f;
 #pragma unroll
     for (int i = 0; i < LN_MAXV; ++i)
-        if (i < nv) {
+        if (ln_has(i, nv, lane, d)) {
             float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, e = v[i].w - mean;
             q += a * a + b * b + c * c + e * e;
         }
@@ -42,17 +47,17 @@ layernorm_kernel(const float *__restrict__ x, int M, int d, const float *__restr
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (row >= M) return;
-    const int nv = d >> 7;  // float4 per lane
+    const int nv = (d + 127) >> 7;  // float4 per lane (the last one partial when d % 128 != 0)
     float4 v[LN_MAXV];
     const float4 *xr = reinterpret_cast<const float4 *>(x + (size_t)row * d);
 #pragma unroll
     for (int i = 0; i < LN_MAXV; ++i)
-        if (i < nv) v[i] = xr[lane + 32 * i];
+        if (ln_has(i, nv, lane, d)) v[i] = xr[lane + 32 * i];
     float mean, rstd;
     ln_stats(v, nv, d, mean, rstd, eps);
 #pragma unroll
     for (int i = 0; i < LN_MAXV; ++i)
-        if (i < nv) {
+        if (ln_has(i, nv, lane, d)) {
             const int c = (lane + 32 * i) * 4;
             const float4 g = *reinterpret_cast<const float4 *>(w1 + c);
             const float4 bb = *reinterpret_cast<const float4 *>(b1 + c);
@@ -67,7 +72,7 @@ layernorm_kernel(const float *__restrict__ x, int M, int d, const float *__restr
     ln_stats(v, nv, d, mean, rstd, eps);
 #pragma unroll
     for (int i = 0; i < LN_MAXV; ++i)
-        if (i < nv) {
+        if (ln_has(i, nv, lane, d)) {
             const int c = (lane + 32 * i) * 4;
             const float4 g = *reinterpret_cast<const float4 *>(w2 + c);
             const float4 bb = *reinterpret_cast<const float4 *>(b2 + c);

@@ -181,6 +181,7 @@ extern "C" {
 pk_status pk_stream_open(pk_engine *e, int32_t n_streams, int32_t max_chunk_samples, int32_t att_context_left, int32_t att_context_right) {
     if (!e || n_streams < 1 || max_chunk_samples < 1 || att_context_left < 1) return PK_ERR_INVALID;
     cudaSetDevice(e->device);
+    if (e->diar) return e->fail(PK_ERR_INVALID, "pk_stream_open: a Sortformer engine diarizes offline only");
     if (e->ss) return e->fail(PK_ERR_INVALID, "pk_stream_open: streams are already open on this engine");
     const pk_config &c = e->cfg;
     if (c.n_durations == 0) return e->fail(PK_ERR_INVALID, "pk_stream_open: streaming decodes a TDT joint; this is an RNN-T model");

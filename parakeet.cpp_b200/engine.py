@@ -36,6 +36,10 @@ class _PkConfig(C.Structure):
         [(n, C.c_int32) for n in ("has_ctc", "joint_prefix_tdt", "max_symbols", "max_batch", "max_samples", "math")]
 
 
+class _PkSortformerConfig(C.Structure):
+    _fields_ = [("enc", _PkConfig)] + [(n, C.c_int32) for n in ("t_hidden", "t_layers", "t_heads", "t_ff", "max_speakers")]
+
+
 class _PkTokens(C.Structure):
     _fields_ = [("cap", C.c_int32), ("ids", C.POINTER(C.c_int32)), ("start", C.POINTER(C.c_int32)),
                 ("end", C.POINTER(C.c_int32)), ("conf", C.POINTER(C.c_float)), ("len", C.POINTER(C.c_int32))]
@@ -75,7 +79,9 @@ EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_co
            "pk_job_begin", "pk_job_append", "pk_nccl_unique_id", "pk_comm_init_rank", "pk_allgather_tokens",
            "pk_job_fetch", "pk_job_stage_pcm", "pk_job_select", "pk_truncated_count",
            "pk_stream_open", "pk_stream_reset", "pk_stream_step", "pk_stream_count", "pk_stage_pcm_rate", "pk_resample_batch",
-           "pk_set_boost", "pk_vocab_max_piece_bytes", "pk_safetensors_probe", "pk_debug_tdt_passes"]
+           "pk_set_boost", "pk_vocab_max_piece_bytes", "pk_safetensors_probe", "pk_debug_tdt_passes",
+           "pk_config_sortformer_117m", "pk_sortformer_create", "pk_sortformer_forward", "pk_diarize_batch", "pk_run_diarize_staged",
+           "pk_fetch_probs", "pk_diar_segments", "pk_kernel_mha", "pk_kernel_speaker_head"]
 
 _lib = None
 
@@ -165,6 +171,16 @@ def load_library():
     L.pk_safetensors_probe.argtypes = [C.c_char_p, C.c_char_p, f32p, C.c_int64, i64p]
     L.pk_stage_pcm_rate.argtypes = [vp, f32p, i64p, C.c_int32, C.c_int32]
     L.pk_resample_batch.argtypes = [vp, f32p, i64p, C.c_int32, C.c_int32, C.c_int32, f32p, i64p]
+    L.pk_config_sortformer_117m.argtypes = [C.POINTER(_PkSortformerConfig)]
+    L.pk_sortformer_create.argtypes = [C.POINTER(_PkSortformerConfig), C.c_char_p, C.c_int, C.POINTER(vp)]
+    L.pk_sortformer_forward.argtypes = [vp, f32p, i32p, C.c_int32, f32p, i32p]
+    L.pk_diarize_batch.argtypes = [vp, f32p, i64p, C.c_int32, f32p, i32p]
+    L.pk_run_diarize_staged.argtypes = [vp]
+    L.pk_fetch_probs.argtypes = [vp, f32p, i32p]
+    L.pk_diar_segments.argtypes = [f32p, C.c_int32, C.c_int32, C.c_float, i32p, f32p, f32p, C.c_int32]
+    L.pk_diar_segments.restype = C.c_int32
+    L.pk_kernel_mha.argtypes = [C.c_int] * 3 + [i32p] + [C.c_int] * 3 + [f32p] * 4 + [i64p]
+    L.pk_kernel_speaker_head.argtypes = [C.c_int] * 4 + [f32p] * 6 + [i64p]
     _lib = L
     return L
 
@@ -290,6 +306,81 @@ def make_tiny_rnnt_config(**kw) -> ModelConfig:
                 max_batch=8, max_samples=64000)
     base.update(kw)
     return ModelConfig(**base)
+
+
+@dataclass
+class SortformerConfig:
+    """SortformerConfig (reference sortformer.hpp:28-41): the NEST encoder (an offline FastConformer under "nest_encoder_."
+    with xscaling and un-normalised features) plus the post-norm transformer and the speaker head.  `encoder` also carries
+    the engine capacity and math."""
+    encoder: ModelConfig
+    t_hidden: int = 192
+    t_layers: int = 18
+    t_heads: int = 8
+    t_ff: int = 768
+    max_speakers: int = 4
+    activity_threshold: float = 0.5
+    name: str = "sortformer-117m"
+
+    @property
+    def mel_bins(self) -> int:
+        return self.encoder.mel_bins
+
+    @property
+    def d_model(self) -> int:
+        return self.encoder.d_model
+
+    @property
+    def n_layers(self) -> int:
+        return self.encoder.n_layers
+
+    @property
+    def max_samples(self) -> int:
+        return self.encoder.max_samples
+
+    def to_c(self) -> _PkSortformerConfig:
+        c = _PkSortformerConfig()
+        c.enc = self.encoder.to_c()
+        c.t_hidden, c.t_layers, c.t_heads, c.t_ff, c.max_speakers = (self.t_hidden, self.t_layers, self.t_heads, self.t_ff,
+                                                                      self.max_speakers)
+        return c
+
+
+def make_sortformer_117m_config(**kw) -> SortformerConfig:   # sortformer.hpp:43-72
+    """kw: capacity and math of the engine (max_batch, max_samples, math)."""
+    enc = dict(mel_bins=128, sub_channels=256, d_model=512, n_layers=17, n_heads=8, ff=2048, vocab=0, pred_hidden=0, lstm_layers=0,
+               joint_hidden=0, durations=(), has_ctc=False, joint_prefix="", max_symbols=0, name="nest-encoder", max_batch=16, max_samples=1440000)
+    enc.update(kw)
+    return SortformerConfig(encoder=ModelConfig(**enc))
+
+
+def make_tiny_sortformer_config(**kw) -> SortformerConfig:
+    """Small test-only Sortformer (not a reference preset): a 2-layer d 128 NEST encoder and a 2-layer post-norm transformer
+    that keeps the preset's head_dim 24 (d 192, 8 heads), ff 384, 4 speakers."""
+    enc = dict(mel_bins=128, sub_channels=64, d_model=128, n_layers=2, n_heads=2, ff=256, vocab=0, pred_hidden=0, lstm_layers=0,
+               joint_hidden=0, durations=(), has_ctc=False, joint_prefix="", max_symbols=0, name="tiny-nest", max_batch=16, max_samples=64000)
+    enc.update(kw)
+    return SortformerConfig(encoder=ModelConfig(**enc), t_layers=2, t_ff=384, name="tiny-sortformer")
+
+
+@dataclass
+class DiarizationSegment:             # sortformer.hpp:20-24
+    speaker_id: int
+    start: float                      # seconds
+    end: float
+
+
+def diar_segments(probs: np.ndarray, threshold: float = 0.5) -> List[DiarizationSegment]:
+    """Sortformer::probs_to_segments (sortformer.cpp:70-113) of one utterance's probs [T][S] (pk_diar_segments)."""
+    L = load_library()
+    p = np.ascontiguousarray(probs, np.float32)
+    T, S = p.shape
+    n = L.pk_diar_segments(_f32p(p), T, S, float(threshold), None, None, None, 0)
+    if n < 0:
+        raise RuntimeError("pk_diar_segments: invalid arguments")
+    spk, st, en = np.zeros(max(n, 1), np.int32), np.zeros(max(n, 1), np.float32), np.zeros(max(n, 1), np.float32)
+    L.pk_diar_segments(_f32p(p), T, S, float(threshold), _i32p(spk), _f32p(st), _f32p(en), n)
+    return [DiarizationSegment(int(spk[i]), float(st[i]), float(en[i])) for i in range(n)]
 
 
 # ------------------------------------------------------------------ result types (timestamp.hpp, transcribe.hpp)
@@ -431,9 +522,10 @@ class Engine:
         self.cfg = cfg
         self.h = C.c_void_p()
         cc = cfg.to_c()
-        st = self.L.pk_engine_create(C.byref(cc), weights_path.encode(), device, C.byref(self.h))
+        create = self.L.pk_sortformer_create if isinstance(cfg, SortformerConfig) else self.L.pk_engine_create
+        st = create(C.byref(cc), weights_path.encode(), device, C.byref(self.h))
         if st != 0:
-            raise RuntimeError(f"pk_engine_create failed ({st}): " + self.L.pk_last_error(None).decode())
+            raise RuntimeError(f"{create.__name__} failed ({st}): " + self.L.pk_last_error(None).decode())
         self.Tmax = self.L.pk_encoder_frames(self.L.pk_mel_frames(cfg.max_samples))
         self.cap = self.token_buffer()[2] - 1       # the engine's token row capacity (2 T'max + 8; RNN-T: max_symbols T'max + 8)
 
@@ -588,6 +680,41 @@ class Engine:
 
     def stream(self) -> int:
         return int(self.L.pk_stream(self.h) or 0)
+
+    # -- Sortformer diarization (an engine made from a SortformerConfig)
+    def _probs(self, lens_out: np.ndarray, out: np.ndarray) -> List[np.ndarray]:
+        offs = np.concatenate([[0], np.cumsum(lens_out)])
+        return [out[offs[i]:offs[i + 1]].copy() for i in range(len(lens_out))]
+
+    def sortformer_forward(self, feats: Sequence[np.ndarray]) -> List[np.ndarray]:
+        """Sortformer::forward per utterance: features [frames][mel_bins] -> sigmoid activities [T'][max_speakers]."""
+        nfr = np.array([f.shape[0] for f in feats], np.int32)
+        buf = np.ascontiguousarray(np.concatenate([np.asarray(f, np.float32) for f in feats], axis=0))
+        M = sum(self.L.pk_encoder_frames(int(n)) for n in nfr)
+        out = np.zeros((M, self.cfg.max_speakers), np.float32)
+        lens = np.zeros(len(feats), np.int32)
+        self._check(self.L.pk_sortformer_forward(self.h, _f32p(buf), _i32p(nfr), len(feats), _f32p(out), _i32p(lens)),
+                    "pk_sortformer_forward")
+        return self._probs(lens, out)
+
+    def diarize_probs(self, pcms: Sequence[np.ndarray]) -> List[np.ndarray]:
+        """The whole path from 16 kHz PCM: activities [T'][max_speakers] per utterance."""
+        buf, off = _pack(pcms)
+        M = sum(self.L.pk_encoder_frames(self.L.pk_mel_frames(len(p))) for p in pcms)
+        out = np.zeros((M, self.cfg.max_speakers), np.float32)
+        lens = np.zeros(len(pcms), np.int32)
+        self._check(self.L.pk_diarize_batch(self.h, _f32p(buf), _i64p(off), len(pcms), _f32p(out), _i32p(lens)), "pk_diarize_batch")
+        return self._probs(lens, out)
+
+    def diarize_batch(self, pcms: Sequence[np.ndarray]) -> List[List[DiarizationSegment]]:
+        """Sortformer::diarize for a batch of PCM utterances."""
+        return [diar_segments(p, self.cfg.activity_threshold) for p in self.diarize_probs(pcms)]
+
+    def run_diarize_staged(self):
+        self._check(self.L.pk_run_diarize_staged(self.h), "pk_run_diarize_staged")
+
+    def fetch_probs(self, out: np.ndarray, lens: np.ndarray):
+        self._check(self.L.pk_fetch_probs(self.h, _f32p(out), _i32p(lens)), "pk_fetch_probs")
 
     # -- phrase boosting on the device (SURVEY.md section 8f row 3)
     def set_boost(self, phrases: Sequence[Sequence[int]], boost: float = 5.0):

@@ -217,3 +217,59 @@ def make_audio(n_samples, seed):
     x = np.clip(x, -0.99, 0.99)
     i16 = np.round(x * 32767.0).astype(np.int16)
     return (i16.astype(F32) / F32(32768.0)).astype(F32)
+
+
+def sortformer_tensor_specs(scfg):
+    """Sortformer (reference sortformer.cpp:42-48, transformer.cpp:9-13): the NEST encoder's tensors under "nest_encoder_.",
+    projection_, transformer_.layers_.{i}, first_hidden_, output_proj_ and the unused hidden_to_spks_.  scfg: an
+    engine.SortformerConfig (or any object with its fields and an `encoder` with those of engine.ModelConfig)."""
+    s = [("nest_" + n, shape, kind) for n, shape, kind in tensor_specs(scfg.encoder) if n.startswith("encoder_.")]
+    d, D, ff, S = scfg.encoder.d_model, scfg.t_hidden, scfg.t_ff, scfg.max_speakers
+    s += [("projection_.weight", (D, d), "w"), ("projection_.bias", (D,), "b")]
+    for i in range(scfg.t_layers):
+        L = f"transformer_.layers_.{i}."
+        for n in ("q_proj", "k_proj", "v_proj", "out_proj"):
+            s += [(L + f"mha_.{n}.weight", (D, D), "wq" if n in ("q_proj", "k_proj") else ("wo" if n == "out_proj" else "w")),
+                  (L + f"mha_.{n}.bias", (D,), "b")]
+        s += [(L + "norm1_.weight", (D,), "g"), (L + "norm1_.bias", (D,), "b"),
+              (L + "fc1_.weight", (ff, D), "w"), (L + "fc1_.bias", (ff,), "b"),
+              (L + "fc2_.weight", (D, ff), "wo"), (L + "fc2_.bias", (D,), "b"),
+              (L + "norm2_.weight", (D,), "g"), (L + "norm2_.bias", (D,), "b")]
+    s += [("first_hidden_.weight", (D, D), "w"), ("first_hidden_.bias", (D,), "b"),
+          ("output_proj_.weight", (S, D), "spk"), ("output_proj_.bias", (S,), "spk_b"),
+          ("hidden_to_spks_.weight", (S, 2 * D), "w"), ("hidden_to_spks_.bias", (S,), "b")]
+    return s
+
+
+def make_sortformer_weights(scfg, seed=0, gain=1.0, out_gain=0.25, spk_gain=4.0, spk_bias=-0.5):
+    """dict name -> ndarray, statistics as make_weights; the speaker head's output_proj_ gets `spk_gain` (zero-mean rows,
+    bias `spk_bias`) so that speaker activities cross 0.5 over time instead of sitting on one side."""
+    import dataclasses
+    rng = np.random.default_rng(seed)
+    # the encoder tensors of make_weights; the ASR decoder it also draws (here of a small dummy shape) is dropped
+    dummy = dataclasses.replace(scfg.encoder, vocab=33, pred_hidden=64, lstm_layers=1, joint_hidden=64, joint_prefix="joint_.",
+                                durations=(), has_ctc=False)
+    enc = make_weights(dummy, seed=seed, gain=gain, out_gain=out_gain)
+    W = {}
+    for name, shape, kind in sortformer_tensor_specs(scfg):
+        if name.startswith("nest_encoder_."):
+            W[name] = enc[name[len("nest_"):]]
+            continue
+        fan_in = int(np.prod(shape[1:])) if len(shape) > 1 else 1
+        if kind == "w":
+            a = rng.standard_normal(shape) * (gain / np.sqrt(fan_in))
+        elif kind == "wq":
+            a = rng.standard_normal(shape) * (2.0 * gain / np.sqrt(fan_in))
+        elif kind == "wo":
+            a = rng.standard_normal(shape) * (out_gain / np.sqrt(fan_in))
+        elif kind == "g":
+            a = 1.0 + 0.1 * rng.standard_normal(shape)
+        elif kind == "spk":
+            a = rng.standard_normal(shape) * (spk_gain / np.sqrt(fan_in))
+            a = a - a.mean(axis=1, keepdims=True)
+        elif kind == "spk_b":
+            a = spk_bias + 0.1 * rng.standard_normal(shape)
+        else:                                # "b"
+            a = 0.1 * rng.standard_normal(shape)
+        W[name] = a.astype(F32)
+    return W
