@@ -420,8 +420,8 @@ typedef struct {
 void pk_config_sortformer_117m(pk_sortformer_config *cfg);
 /* An engine in diarization mode.  Required keys: nest_encoder_.*, projection_, transformer_.layers_.{i}.{norm1_, mha_.{q,k,v,out}_proj,
  * norm2_, fc1_, fc2_}, first_hidden_, output_proj_ (hidden_to_spks_ is not used and not required).  On it pk_mel, pk_encode
- * (the NEST encoder output), pk_stage_pcm, the profile calls and pk_last_error work; the decode, boosting and streaming entry
- * points return PK_ERR_INVALID. */
+ * (the NEST encoder output), pk_stage_pcm, the profile calls and pk_last_error work; the decode, boosting and ASR streaming
+ * (pk_stream_*) entry points return PK_ERR_INVALID.  Its streams are the pk_diar_stream_* calls below. */
 pk_status pk_sortformer_create(const pk_sortformer_config *cfg, const char *safetensors_path, int device, pk_engine **out);
 /* Sortformer::forward on a batch of features (packed (sum frames_i, mel_bins), as pk_mel returns them): probs_out packed
  * (sum T'_i, max_speakers) sigmoid activities, t_out[n_utt] = T'_i (may be NULL). */
@@ -436,6 +436,34 @@ pk_status pk_fetch_probs(pk_engine *e, float *probs_out, int32_t *t_out);
  * p > threshold; a segment is [start frame, last active frame] in seconds (frame * 0.08 s); segments sorted by start, equal
  * starts by speaker id.  Writes at most cap segments; returns their full number, or -1 on invalid arguments. */
 int32_t pk_diar_segments(const float *probs, int32_t T, int32_t S, float threshold, int32_t *spk, float *start, float *end, int32_t cap);
+/* Streaming diarization: Sortformer::diarize_chunk (sortformer.cpp:124-150) with one EncoderCache and AOSCCache per stream,
+ * n_streams streams in lock step on a Sortformer engine (the pk_stream_* conventions).  Per stream and step: the chunk's own
+ * centred log-mel without normalisation (preprocess_audio(chunk, {n_mels = mel_bins, normalize = false}); nothing carries
+ * over between chunks), the NEST encoder's forward_chunk (leftover mel frames, K/V rings of att_context_left rows, conv
+ * caches), then projection_ -> transformer_ -> speaker head on THIS chunk's encoder rows only (no context across chunks, as
+ * in the reference), and the AOSC update (a speaker arrives the first time its p > 0.5; within a frame in index order).
+ *   pk_diar_stream_open : capacity as pk_stream_open: n_streams <= max_batch, att_context_left + encoder frames per chunk
+ *                         <= the engine's encoder-frame capacity (PK_ERR_CAPACITY otherwise).  On an ASR engine: PK_ERR_INVALID.
+ *   pk_diar_stream_step : stream s receives pcm[offsets[s] .. offsets[s+1]) (16 kHz; empty = no input this step; a chunk
+ *                         over max_chunk_samples is PK_ERR_CAPACITY, a 1-sample chunk PK_ERR_INVALID: the reference's
+ *                         reflect pad does not terminate there).  probs_out packed (sum C_s, max_speakers) sigmoid
+ *                         activities of this step, n_out[s] = C_s (0: the reference returns {} and the AOSC is not
+ *                         updated), frame_base_out[s] = the absolute encoder frame of the stream's first row (probs are
+ *                         chunk-local: segments restart at frame 0 in every chunk).  enc_out (may be NULL): debug tap of
+ *                         the NEST encoder rows, packed (sum C_s, d_model).  Any output pointer may be NULL.
+ *   pk_diar_stream_step_feats : the same from host features, stream s = n_frames[s] rows of feats packed (sum, mel_bins)
+ *                         (diarize_chunk's own input; n_frames[s] <= 1 + max_chunk_samples / 160).
+ *   pk_diar_stream_speakers : AOSCCache::speaker_order of one stream; writes at most cap ids, returns their number (-1 on
+ *                         invalid arguments).
+ *   pk_diar_stream_reset : a fresh EncoderCache and AOSCCache::reset for one stream (-1: all). */
+pk_status pk_diar_stream_open(pk_engine *e, int32_t n_streams, int32_t max_chunk_samples, int32_t att_context_left);
+pk_status pk_diar_stream_reset(pk_engine *e, int32_t stream);
+pk_status pk_diar_stream_step(pk_engine *e, const float *pcm, const int64_t *offsets, float *probs_out, int32_t *n_out,
+                              int32_t *frame_base_out, float *enc_out);
+pk_status pk_diar_stream_step_feats(pk_engine *e, const float *feats, const int32_t *n_frames, float *probs_out, int32_t *n_out,
+                                    int32_t *frame_base_out, float *enc_out);
+int32_t pk_diar_stream_speakers(const pk_engine *e, int32_t stream, int32_t *order, int32_t cap);
+int32_t pk_diar_stream_count(const pk_engine *e);
 /* Kernel test hooks (conventions of the pk_kernel_* hooks above).  pk_kernel_mha: the transformer attention on qkv [rows_total][3 d]
  * fp32 (q | k | v), head_dim 24 only (else PK_ERR_INVALID); ctx [rows_total][d] in ctx_f32 with PK_MATH_FP32, else ctx_hi and,
  * with PK_MATH_BF16X3, ctx_lo.  pk_kernel_speaker_head: x [M][D], w1 [D][D], b1 [D], w2 [S][D], b2 [S] -> probs [M][S]. */

@@ -1076,7 +1076,7 @@ static pk_status create_engine(const pk_config &c, const pk_sortformer_config *s
     if (const char *ev = getenv("PK_GRAPH")) e->use_graphs = atoi(ev) != 0;
     if (const char *ev = getenv("PK_ATTN_TC")) e->attn_tc = atoi(ev) != 0;
     if (const char *ev = getenv("PK_ATTN_UMMA")) e->attn_wgmma = atoi(ev) != 0;
-    if (const char *ev = getenv("PK_GEMM_SKINNY")) e->skinny = atoi(ev) != 0;
+    if (const char *ev = getenv("PK_GEMM_SKINNY")) e->skinny = e->stream_skinny = atoi(ev) != 0;
     if (const char *ev = getenv("PK_FUSE_LN")) e->fuse_ln = atoi(ev) != 0;
     if (const char *ev = getenv("PK_GEMM_CLUSTER")) e->gemm_cluster = atoi(ev);
     if (const char *ev = getenv("PK_LN_MCAST")) e->ln_mcast = atoi(ev) != 0;

@@ -275,6 +275,7 @@ struct pk_engine {
     bool fuse_ln = false;                      // PK_FUSE_LN=1: LayerNorm in the epilogue of the GEMM that produces its input
     // few-row GEMMs (M <= 128: streaming steps, short utterances) go to gemm_skinny.cu (PK_GEMM_SKINNY=0: never)
     bool skinny = true;
+    bool stream_skinny = true;                 // the same for the steps of Sortformer streams (offline diarization keeps skinny off)
     float *skinny_ws = nullptr;
     size_t skinny_ws_floats = 0;
     unsigned int *skinny_tickets = nullptr;
@@ -285,7 +286,7 @@ struct pk_engine {
     pk_status run_graphed(const std::string &key, const std::function<pk_status()> &body);
     pk_status run_subsample_tail(bool with_first_ln = false);
     pk_status run_encoder(float *sub_out_host, float *layers_out_host);
-    // streaming eou path (stream_engine.cu)
+    // streaming eou path (stream_engine.cu); on a Sortformer engine the streams of pk_diar_stream_open
     struct StreamSet *ss = nullptr;
     pk_status run_stream_layers();
     pk_status run_stream_decode();

@@ -53,6 +53,10 @@ void launch_stream_prep(const float *chunk, const StreamPlan *plan, StreamState 
                         int n_mels, cudaStream_t s);
 void launch_stream_post(const float *chunk, const StreamPlan *plan, StreamState st, int n_streams, const float *ssig,
                         const float *mel_in, int n_mels, float *feats, cudaStream_t s);
+// Sortformer streams: per stream, [melq (plan.left rows) | mel_new rows plan.min_off .. + plan.nf] -> the first plan.take
+// rows to feats row plan.feat_off, the rest (< 8) back into melq.  No sample overlap, no pre-emphasis carry.
+void launch_diar_stream_join(const StreamPlan *plan, const float *mel_new, float *melq, int n_streams, int n_mels, float *feats,
+                             cudaStream_t s);
 bool launch_stream_attention(const float *qkv, int ld_qkv, const int32_t *row_off, const int32_t *act_stream, int n_active,
                              int max_C, const int32_t *cache_len, const int32_t *ring_start, float *kc, float *vc, int L,
                              int n_heads, int hd, int d_model, const float *pp, int tmax, const float *bu, const float *bv,

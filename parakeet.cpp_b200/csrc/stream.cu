@@ -65,6 +65,31 @@ __global__ void stream_post_kernel(const float *__restrict__ chunk, const Stream
     for (int i = threadIdx.x; i < rest * n_mels; i += blockDim.x) q[i] = mi[(size_t)p.take * n_mels + i];
 }
 
+// Sortformer streams (Sortformer::diarize_chunk, sortformer.cpp:124-150): every chunk's log-mel is computed on its own
+// (centred STFT), so no samples or pre-emphasis carry over; only CausalConvSubsampling's leftover frames
+// (streaming_encoder.cpp:348-385) do.  Joined = [queue (left rows) | this chunk's nf rows at mel_new row p.min_off]: the
+// first `take` rows go to the packed encoder input, the rest (< 8) back into the queue.
+__global__ void diar_stream_join_kernel(const StreamPlan *__restrict__ plan, const float *__restrict__ mel_new,
+                                        float *__restrict__ melq, int n_mels, float *__restrict__ feats) {
+    pdl_wait();
+    pdl_trigger();
+    const int s = blockIdx.x;
+    const StreamPlan p = plan[s];
+    float *q = melq + (size_t)s * 8 * n_mels;
+    const float *nw = mel_new + (size_t)p.min_off * n_mels;
+    const int lq = p.left * n_mels;
+    if (p.take > 0) {
+        float *f = feats + (size_t)p.feat_off * n_mels;
+        for (int i = threadIdx.x; i < p.take * n_mels; i += blockDim.x) f[i] = i < lq ? q[i] : nw[i - lq];
+        __syncthreads();                                    // the queue is read above, rewritten below
+        const int rest = p.left + p.nf - p.take;            // < 8, all from this chunk (take >= 8 > left)
+        const float *src = nw + (size_t)(p.take - p.left) * n_mels;
+        for (int i = threadIdx.x; i < rest * n_mels; i += blockDim.x) q[i] = src[i];
+    } else {
+        for (int i = threadIdx.x; i < p.nf * n_mels; i += blockDim.x) q[lq + i] = nw[i];
+    }
+}
+
 // ---- cached attention (streaming_encoder.cpp:160-272) ----------------------------------------------------------
 // One block per (head, active stream).  Keys = [cached rows (ring, oldest first) | this chunk's rows]; scores
 //     ((q_i + u) . k_j + (q_i + v) . PP[pos_j]) / sqrt(hd)
@@ -196,6 +221,11 @@ void launch_stream_prep(const float *chunk, const StreamPlan *plan, StreamState 
 void launch_stream_post(const float *chunk, const StreamPlan *plan, StreamState st, int n_streams, const float *ssig,
                         const float *mel_in, int n_mels, float *feats, cudaStream_t s) {
     launch_pdl(stream_post_kernel, dim3(n_streams), dim3(256), 0, s, chunk, plan, st, ssig, mel_in, n_mels, feats);
+}
+
+void launch_diar_stream_join(const StreamPlan *plan, const float *mel_new, float *melq, int n_streams, int n_mels, float *feats,
+                             cudaStream_t s) {
+    launch_pdl(diar_stream_join_kernel, dim3(n_streams), dim3(256), 0, s, plan, mel_new, melq, n_mels, feats);
 }
 
 size_t stream_attention_smem(int L, int Cmax, int hd) { return sizeof(float) * ((size_t)2 * (L + Cmax) * (hd + 1) + 2 * hd + L + Cmax); }

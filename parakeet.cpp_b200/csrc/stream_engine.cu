@@ -40,6 +40,12 @@ struct StreamSet {
     float *h_chunk = nullptr;                                  // pinned staging of the chunk samples
     cudaEvent_t ev_up = nullptr;                               // uploads of the previous step consumed
     size_t state_bytes = 0;
+    // Sortformer streams (pk_diar_stream_open): no sample overlap, LSTM or token state; h_meta [0, S] holds the mel frame
+    // offsets of the step's chunks, d_chunk / d_sig_off the packed PCM and its offsets.
+    bool diar = false;
+    float *mel_new = nullptr, *h_mel = nullptr;                // this step's log-mel frames [S * nf_max][mel] (h_mel pinned)
+    std::vector<uint64_t> spk_seen;                            // AOSCCache::speaker_active_ (max_speakers <= 64)
+    std::vector<std::vector<int32_t>> arrival;                 // AOSCCache::arrival_order_
 };
 
 namespace {
@@ -51,7 +57,7 @@ inline int enc_frames(int mel_frames) { return conv_len(conv_len(conv_len(mel_fr
 // Conformer blocks on the packed chunk rows (streaming_encoder.cpp:430-472): ffn1 -> cached attention -> cached conv ->
 // ffn2 -> LayerNorm, the same GEMM / LayerNorm kernels as the offline encoder (engine.cu run_encoder).
 pk_status pk_engine::run_stream_layers() {
-    StreamSet &s = *ss;
+    StreamSet &s = *ss;   // ASR or Sortformer streams: the same encoder state
     const pk_config &c = cfg;
     const int d = c.d_model, H = c.n_heads, hd = d / H;
     const int n_act = (int)s.act.size();
@@ -181,7 +187,7 @@ extern "C" {
 pk_status pk_stream_open(pk_engine *e, int32_t n_streams, int32_t max_chunk_samples, int32_t att_context_left, int32_t att_context_right) {
     if (!e || n_streams < 1 || max_chunk_samples < 1 || att_context_left < 1) return PK_ERR_INVALID;
     cudaSetDevice(e->device);
-    if (e->diar) return e->fail(PK_ERR_INVALID, "pk_stream_open: a Sortformer engine diarizes offline only");
+    if (e->diar) return e->fail(PK_ERR_INVALID, "pk_stream_open: a Sortformer engine opens its streams with pk_diar_stream_open");
     if (e->ss) return e->fail(PK_ERR_INVALID, "pk_stream_open: streams are already open on this engine");
     const pk_config &c = e->cfg;
     if (c.n_durations == 0) return e->fail(PK_ERR_INVALID, "pk_stream_open: streaming decodes a TDT joint; this is an RNN-T model");
@@ -226,6 +232,7 @@ pk_status pk_stream_open(pk_engine *e, int32_t n_streams, int32_t max_chunk_samp
 pk_status pk_stream_reset(pk_engine *e, int32_t stream) {
     if (!e || !e->ss) return PK_ERR_INVALID;
     cudaSetDevice(e->device);
+    if (e->diar) return e->fail(PK_ERR_INVALID, "pk_stream_reset: a Sortformer engine's streams reset with pk_diar_stream_reset");
     StreamSet &s = *e->ss;
     const pk_config &c = e->cfg;
     if (stream < -1 || stream >= s.S) return e->fail(PK_ERR_INVALID, "pk_stream_reset: bad stream index");
@@ -267,6 +274,7 @@ pk_status pk_stream_step(pk_engine *e, const float *pcm, const int64_t *offsets,
                          float *enc_out, int32_t *n_enc) {
     if (!e || !e->ss || !offsets || (!pcm && offsets[e->ss->S] > offsets[0])) return PK_ERR_INVALID;
     cudaSetDevice(e->device);
+    if (e->diar) return e->fail(PK_ERR_INVALID, "pk_stream_step: a Sortformer engine's streams step with pk_diar_stream_step");
     StreamSet &s = *e->ss;
     const pk_config &c = e->cfg;
     const int S = s.S;
@@ -391,7 +399,246 @@ pk_status pk_stream_step(pk_engine *e, const float *pcm, const int64_t *offsets,
     return e->fetch(out);
 }
 
-int32_t pk_stream_count(const pk_engine *e) { return (e && e->ss) ? e->ss->S : 0; }
+int32_t pk_stream_count(const pk_engine *e) { return (e && e->ss && !e->diar) ? e->ss->S : 0; }
+
+// ===================================================================== Sortformer streams (sortformer.cpp:124-150)
+// Sortformer::diarize_chunk for S streams in lock step.  Per stream and step: the chunk's own centred log-mel without
+// normalisation (preprocess_audio(chunk, {n_mels = mel_bins, normalize = false}), no state across chunks), the NEST encoder's
+// forward_chunk (leftover frames, K/V rings and conv caches of every layer), then projection_ -> transformer_ -> speaker head
+// on THIS chunk's encoder rows only (each active stream is one utterance of the packed step), and the AOSC update on the host.
+
+pk_status pk_diar_stream_open(pk_engine *e, int32_t n_streams, int32_t max_chunk_samples, int32_t att_context_left) {
+    if (!e || n_streams < 1 || max_chunk_samples < 1 || att_context_left < 1) return PK_ERR_INVALID;
+    cudaSetDevice(e->device);
+    if (!e->diar) return e->fail(PK_ERR_INVALID, "pk_diar_stream_open: not a Sortformer engine (pk_sortformer_create)");
+    if (e->ss) return e->fail(PK_ERR_INVALID, "pk_diar_stream_open: streams are already open on this engine");
+    const pk_config &c = e->cfg;
+    auto s = std::make_unique<StreamSet>();
+    s->diar = true;
+    s->S = n_streams; s->L = att_context_left; s->R = 0; s->max_chunk = max_chunk_samples;
+    s->nf_max = 1 + max_chunk_samples / 160;                   // centred STFT: 1 + n / 160 frames per chunk
+    s->take_max = ((7 + s->nf_max) / 8) * 8;                   // + up to 7 leftover frames
+    s->c_max = enc_frames(s->take_max);
+    if (n_streams > e->Bmax) return e->fail(PK_ERR_CAPACITY, "pk_diar_stream_open: more streams than pk_config.max_batch");
+    if (s->take_max > e->Fmax || s->L + s->c_max > e->Tmax)
+        return e->fail(PK_ERR_CAPACITY, "pk_diar_stream_open: pk_config.max_samples too small (needs encoder frames >= att_context_left + frames per chunk)");
+    const int S = n_streams, d = c.d_model, nl = c.n_layers;
+    s->left.assign(S, 0); s->cache_len.assign(S, 0); s->ring_start.assign(S, 0); s->frame_base.assign(S, 0);
+    s->spk_seen.assign(S, 0); s->arrival.assign(S, {});
+    s->st.melq = e->dalloc<float>((size_t)S * 8 * c.mel_bins);
+    s->kc = e->dalloc<float>((size_t)nl * S * s->L * d);
+    s->vc = e->dalloc<float>((size_t)nl * S * s->L * d);
+    s->convc = e->dalloc<float>((size_t)nl * S * (c.conv_kernel - 1) * d);
+    s->d_chunk = e->dalloc<float>((size_t)S * max_chunk_samples + 8);
+    s->mel_new = e->dalloc<float>((size_t)S * s->nf_max * c.mel_bins);
+    s->d_plan = e->dalloc<StreamPlan>(S);
+    s->d_sig_off = e->dalloc<int64_t>(S + 1);
+    s->d_meta = e->dalloc<int32_t>((size_t)7 * S + 8);
+    if (!s->st.melq || !s->kc || !s->vc || !s->convc || !s->d_chunk || !s->mel_new || !s->d_plan || !s->d_sig_off || !s->d_meta)
+        return e->fail(PK_ERR_CUDA, "cudaMalloc failed (diarization stream state)");
+    if (cudaMallocHost(&s->h_plan, sizeof(StreamPlan) * S) != cudaSuccess || cudaMallocHost(&s->h_sig_off, sizeof(int64_t) * (S + 1)) != cudaSuccess ||
+        cudaMallocHost(&s->h_meta, sizeof(int32_t) * (7 * S + 8)) != cudaSuccess ||
+        cudaMallocHost(&s->h_chunk, sizeof(float) * ((size_t)S * max_chunk_samples + 8)) != cudaSuccess ||
+        cudaMallocHost(&s->h_mel, sizeof(float) * (size_t)S * s->nf_max * c.mel_bins) != cudaSuccess ||
+        cudaEventCreateWithFlags(&s->ev_up, cudaEventDisableTiming) != cudaSuccess) {
+        e->ss = s.release();                                    // frees what was allocated
+        pk_stream_free(e);
+        return e->fail(PK_ERR_CUDA, "cudaMallocHost failed (diarization stream staging)");
+    }
+    e->ss = s.release();
+    return pk_diar_stream_reset(e, -1);
+}
+
+// A fresh EncoderCache and AOSCCache::reset (sortformer.cpp:35-38) for one stream (or all: stream = -1)
+pk_status pk_diar_stream_reset(pk_engine *e, int32_t stream) {
+    if (!e) return PK_ERR_INVALID;
+    cudaSetDevice(e->device);
+    if (!e->diar || !e->ss) return e->fail(PK_ERR_INVALID, "pk_diar_stream_reset: no Sortformer streams open (pk_diar_stream_open)");
+    StreamSet &s = *e->ss;
+    const pk_config &c = e->cfg;
+    if (stream < -1 || stream >= s.S) return e->fail(PK_ERR_INVALID, "pk_diar_stream_reset: bad stream index");
+    const int s0 = stream < 0 ? 0 : stream, s1 = stream < 0 ? s.S : stream + 1;
+    cudaEventSynchronize(s.ev_up);
+    cudaError_t ce = cudaSuccess;
+    for (int i = s0; i < s1 && ce == cudaSuccess; ++i) {
+        s.left[i] = s.cache_len[i] = s.ring_start[i] = s.frame_base[i] = 0;
+        s.spk_seen[i] = 0;
+        s.arrival[i].clear();
+        // conv caches start as zeros (streaming_encoder.cpp:52-56); K / V rings and the mel queue are empty (lengths 0)
+        for (int l = 0; l < c.n_layers && ce == cudaSuccess; ++l)
+            ce = cudaMemsetAsync(s.convc + ((size_t)l * s.S + i) * (c.conv_kernel - 1) * c.d_model, 0,
+                                 sizeof(float) * (c.conv_kernel - 1) * c.d_model, e->stream);
+    }
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
+    if (ce != cudaSuccess) return e->fail(PK_ERR_CUDA, std::string("pk_diar_stream_reset: ") + cudaGetErrorString(ce));
+    return PK_OK;
+}
+
+namespace {
+
+// One step from PCM (pcm / offsets) or from host features (feats / n_frames).
+pk_status diar_stream_step(pk_engine *e, const float *pcm, const int64_t *offsets, const float *feats, const int32_t *n_frames,
+                           float *probs_out, int32_t *n_out, int32_t *frame_base_out, float *enc_out) {
+    const char *fn = feats ? "pk_diar_stream_step_feats" : "pk_diar_stream_step";
+    if (!e) return PK_ERR_INVALID;
+    cudaSetDevice(e->device);
+    if (!e->diar || !e->ss) return e->fail(PK_ERR_INVALID, std::string(fn) + ": no Sortformer streams open (pk_diar_stream_open)");
+    StreamSet &s = *e->ss;
+    const pk_config &c = e->cfg;
+    const int S = s.S, nm = c.mel_bins, SP = e->sf.max_speakers;
+    if (pk_status g = e->gemm_err) return g;
+    cudaEventSynchronize(s.ev_up);                 // the previous step has consumed the pinned staging buffers
+    // ---- the plan: pure integer bookkeeping, checked for every stream before any state changes
+    int32_t *m_fo = s.h_meta, *m_act = s.h_meta + 2 * S, *m_cl = s.h_meta + 3 * S, *m_rs = s.h_meta + 4 * S, *m_ro = s.h_meta + 6 * S;
+    s.act.clear(); s.take.clear(); s.nC.clear();
+    m_fo[0] = 0; m_ro[0] = 0;
+    int64_t soff = 0;
+    int foff = 0, max_nf = 0;
+    std::vector<int32_t> new_left(S);
+    for (int i = 0; i < S; ++i) {
+        int nf;
+        if (feats) {
+            nf = n_frames ? n_frames[i] : -1;
+            if (nf < 0) return e->fail(PK_ERR_INVALID, std::string(fn) + ": n_frames missing or negative");
+            if (nf > s.nf_max) return e->fail(PK_ERR_CAPACITY, std::string(fn) + ": more frames than a chunk of max_chunk_samples makes");
+        } else {
+            const int64_t n = offsets[i + 1] - offsets[i];
+            if (n < 0 || n > s.max_chunk) return e->fail(PK_ERR_CAPACITY, std::string(fn) + ": chunk longer than max_chunk_samples");
+            // axiom's reflect pad never terminates on a 1-sample signal (operations.cpp:2217-2227, DESIGN.md)
+            if (n == 1) return e->fail(PK_ERR_INVALID, std::string(fn) + ": a 1-sample chunk cannot be reflect-padded (the reference does not return)");
+            nf = n > 0 ? (int)(1 + n / 160) : 0;
+            s.h_sig_off[i] = soff;
+            if (n > 0) memcpy(s.h_chunk + soff, pcm + offsets[i], sizeof(float) * n);
+            soff += n;
+        }
+        StreamPlan &p = s.h_plan[i];
+        memset(&p, 0, sizeof(p));
+        p.nf = nf; p.left = s.left[i]; p.min_off = m_fo[i];
+        const int frames = p.left + nf;
+        p.take = (frames / 8) * 8;
+        p.feat_off = foff;
+        new_left[i] = frames - p.take;
+        m_fo[i + 1] = m_fo[i] + nf;
+        m_cl[i] = s.cache_len[i]; m_rs[i] = s.ring_start[i];
+        int C = 0;
+        if (p.take > 0) {
+            C = enc_frames(p.take);
+            s.act.push_back(i); s.take.push_back(p.take); s.nC.push_back(C);
+            foff += p.take;
+        }
+        m_ro[i + 1] = m_ro[i] + C;
+        max_nf = std::max(max_nf, nf);
+    }
+    s.h_sig_off[S] = soff;
+    const int n_act = (int)s.act.size();
+    for (int a = 0; a < n_act; ++a) m_act[a] = s.act[a];
+    if (feats && m_fo[S] > 0) memcpy(s.h_mel, feats, sizeof(float) * (size_t)m_fo[S] * nm);
+    cudaStream_t st = e->stream;
+    cudaError_t ce = cudaMemcpyAsync(s.d_plan, s.h_plan, sizeof(StreamPlan) * S, cudaMemcpyHostToDevice, st);
+    if (ce == cudaSuccess) ce = cudaMemcpyAsync(s.d_meta, s.h_meta, sizeof(int32_t) * (7 * S + 1), cudaMemcpyHostToDevice, st);
+    if (ce == cudaSuccess && !feats) ce = cudaMemcpyAsync(s.d_sig_off, s.h_sig_off, sizeof(int64_t) * (S + 1), cudaMemcpyHostToDevice, st);
+    if (ce == cudaSuccess && soff > 0) ce = cudaMemcpyAsync(s.d_chunk, s.h_chunk, sizeof(float) * soff, cudaMemcpyHostToDevice, st);
+    if (ce == cudaSuccess && feats && m_fo[S] > 0)
+        ce = cudaMemcpyAsync(s.mel_new, s.h_mel, sizeof(float) * (size_t)m_fo[S] * nm, cudaMemcpyHostToDevice, st);
+    if (ce == cudaSuccess) ce = cudaEventRecord(s.ev_up, st);
+    if (ce != cudaSuccess) return e->fail(PK_ERR_CUDA, std::string(fn) + " upload: " + cudaGetErrorString(ce));
+    // ---- front end: every chunk's centred log-mel in one launch (K1 of the offline front end), then the queue join
+    if (!feats && max_nf > 0) {
+        pk_engine::Scope sc(e, pk_engine::CAT_MEL);
+        launch_mel(s.d_chunk, s.d_sig_off, s.d_meta, S, max_nf, nm, e->mel_tb, nullptr, s.mel_new, nullptr, st, false);
+        ++e->launches;
+    }
+    launch_diar_stream_join(s.d_plan, s.mel_new, s.st.melq, S, nm, e->feats, st);
+    ++e->launches;
+    // ---- host state of the next step
+    std::vector<int32_t> base(s.frame_base);
+    for (int i = 0; i < S; ++i) {
+        s.left[i] = new_left[i];
+        const int C = m_ro[i + 1] - m_ro[i], kv = s.cache_len[i] + C;
+        if (kv > s.L) s.ring_start[i] = (s.ring_start[i] + kv - s.L) % s.L;
+        s.cache_len[i] = std::min(kv, s.L);
+        s.frame_base[i] += C;
+    }
+    if (n_out) for (int i = 0; i < S; ++i) n_out[i] = m_ro[i + 1] - m_ro[i];
+    if (frame_base_out) for (int i = 0; i < S; ++i) frame_base_out[i] = base[i];
+    if (n_act == 0) {                              // CausalConvSubsampling returned nothing for every stream: no AOSC update
+        ce = cudaStreamSynchronize(st);
+        return ce == cudaSuccess ? PK_OK : e->fail(PK_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(ce));
+    }
+    // ---- encoder, transformer and speaker head on the active streams' rows
+    pk_status ps;
+    if ((ps = e->set_batch_shapes(s.take.data(), nullptr, n_act))) return ps;
+    if ((ps = e->upload_shapes())) return ps;
+    auto body = [e, enc_out, st]() -> pk_status {
+        const bool sk = e->skinny;
+        e->skinny = e->stream_skinny;              // few rows per step: the weight-streaming GEMM
+        pk_status q = e->run_conv1();
+        if (!q) q = e->run_subsample_tail();
+        if (!q) q = e->run_stream_layers();
+        if (!q && enc_out) {
+            cudaError_t c2 = cudaMemcpyAsync(enc_out, e->x, sizeof(float) * (size_t)e->M * e->cfg.d_model, cudaMemcpyDeviceToHost, st);
+            if (c2 != cudaSuccess) q = e->fail(PK_ERR_CUDA, std::string("pk_diar_stream_step tap: ") + cudaGetErrorString(c2));
+        }
+        if (!q) q = e->run_diar_head();
+        e->skinny = sk;
+        return q;
+    };
+    if (enc_out) {
+        ps = body();                               // (debug tap: plain launches)
+    } else {
+        // every kernel argument depends only on which streams take how many frames: one graph per pattern ('D': not an
+        // offline diarization key 'd' nor an ASR stream key 's')
+        std::string key(1, 'D');
+        key.append(reinterpret_cast<const char *>(s.act.data()), s.act.size() * sizeof(int32_t));
+        key.append(reinterpret_cast<const char *>(s.take.data()), s.take.size() * sizeof(int32_t));
+        ps = e->run_graphed(key, body);
+    }
+    if (ps) return ps;
+    if (e->gemm_err) return e->gemm_err;
+    const size_t np = (size_t)e->M * SP;
+    ce = cudaMemcpyAsync(e->h_probs, e->probs, np * sizeof(float), cudaMemcpyDeviceToHost, st);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+    if (ce != cudaSuccess) return e->fail(PK_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(ce));
+    if (probs_out) memcpy(probs_out, e->h_probs, np * sizeof(float));
+    // AOSCCache::update (sortformer.cpp:15-31): a speaker arrives the first time p > 0.5; within a frame in index order
+    for (int a = 0; a < n_act; ++a) {
+        const int i = s.act[a];
+        for (int t = m_ro[i]; t < m_ro[i + 1]; ++t)
+            for (int k = 0; k < SP; ++k)
+                if (e->h_probs[(size_t)t * SP + k] > 0.5f && !(s.spk_seen[i] >> k & 1)) {
+                    s.spk_seen[i] |= 1ull << k;
+                    s.arrival[i].push_back(k);
+                }
+    }
+    return PK_OK;
+}
+
+}  // namespace
+
+pk_status pk_diar_stream_step(pk_engine *e, const float *pcm, const int64_t *offsets, float *probs_out, int32_t *n_out,
+                              int32_t *frame_base_out, float *enc_out) {
+    if (!e || !offsets || (e->ss && !pcm && offsets[e->ss->S] > offsets[0])) return PK_ERR_INVALID;
+    return diar_stream_step(e, pcm, offsets, nullptr, nullptr, probs_out, n_out, frame_base_out, enc_out);
+}
+
+pk_status pk_diar_stream_step_feats(pk_engine *e, const float *feats, const int32_t *n_frames, float *probs_out, int32_t *n_out,
+                                    int32_t *frame_base_out, float *enc_out) {
+    if (!e || !n_frames) return PK_ERR_INVALID;
+    if (!feats && e->ss)
+        for (int i = 0; i < e->ss->S; ++i)
+            if (n_frames[i] > 0) return e->fail(PK_ERR_INVALID, "pk_diar_stream_step_feats: frames without features");
+    static const float none = 0.f;
+    return diar_stream_step(e, nullptr, nullptr, feats ? feats : &none, n_frames, probs_out, n_out, frame_base_out, enc_out);
+}
+
+int32_t pk_diar_stream_speakers(const pk_engine *e, int32_t stream, int32_t *order, int32_t cap) {
+    if (!e || !e->diar || !e->ss || stream < 0 || stream >= e->ss->S || cap < 0 || (cap > 0 && !order)) return -1;
+    const std::vector<int32_t> &a = e->ss->arrival[stream];
+    for (size_t i = 0; i < a.size() && (int64_t)i < cap; ++i) order[i] = a[i];
+    return (int32_t)a.size();
+}
+
+int32_t pk_diar_stream_count(const pk_engine *e) { return (e && e->diar && e->ss) ? e->ss->S : 0; }
 
 }  // extern "C"
 
@@ -402,6 +649,7 @@ void pk_stream_free(pk_engine *e) {
     if (s->h_sig_off) cudaFreeHost(s->h_sig_off);
     if (s->h_meta) cudaFreeHost(s->h_meta);
     if (s->h_chunk) cudaFreeHost(s->h_chunk);
+    if (s->h_mel) cudaFreeHost(s->h_mel);
     if (s->ev_up) cudaEventDestroy(s->ev_up);
     delete s;
     e->ss = nullptr;

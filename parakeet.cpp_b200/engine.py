@@ -81,7 +81,9 @@ EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_co
            "pk_stream_open", "pk_stream_reset", "pk_stream_step", "pk_stream_count", "pk_stage_pcm_rate", "pk_resample_batch",
            "pk_set_boost", "pk_vocab_max_piece_bytes", "pk_safetensors_probe", "pk_debug_tdt_passes",
            "pk_config_sortformer_117m", "pk_sortformer_create", "pk_sortformer_forward", "pk_diarize_batch", "pk_run_diarize_staged",
-           "pk_fetch_probs", "pk_diar_segments", "pk_kernel_mha", "pk_kernel_speaker_head"]
+           "pk_fetch_probs", "pk_diar_segments", "pk_kernel_mha", "pk_kernel_speaker_head",
+           "pk_diar_stream_open", "pk_diar_stream_reset", "pk_diar_stream_step", "pk_diar_stream_step_feats", "pk_diar_stream_speakers",
+           "pk_diar_stream_count"]
 
 _lib = None
 
@@ -181,6 +183,14 @@ def load_library():
     L.pk_diar_segments.restype = C.c_int32
     L.pk_kernel_mha.argtypes = [C.c_int] * 3 + [i32p] + [C.c_int] * 3 + [f32p] * 4 + [i64p]
     L.pk_kernel_speaker_head.argtypes = [C.c_int] * 4 + [f32p] * 6 + [i64p]
+    L.pk_diar_stream_open.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32]
+    L.pk_diar_stream_reset.argtypes = [vp, C.c_int32]
+    L.pk_diar_stream_step.argtypes = [vp, f32p, i64p, f32p, i32p, i32p, f32p]
+    L.pk_diar_stream_step_feats.argtypes = [vp, f32p, i32p, f32p, i32p, i32p, f32p]
+    L.pk_diar_stream_speakers.argtypes = [vp, C.c_int32, i32p, C.c_int32]
+    L.pk_diar_stream_speakers.restype = C.c_int32
+    L.pk_diar_stream_count.argtypes = [vp]
+    L.pk_diar_stream_count.restype = C.c_int32
     _lib = L
     return L
 
@@ -381,6 +391,31 @@ def diar_segments(probs: np.ndarray, threshold: float = 0.5) -> List[Diarization
     spk, st, en = np.zeros(max(n, 1), np.int32), np.zeros(max(n, 1), np.float32), np.zeros(max(n, 1), np.float32)
     L.pk_diar_segments(_f32p(p), T, S, float(threshold), _i32p(spk), _f32p(st), _f32p(en), n)
     return [DiarizationSegment(int(spk[i]), float(st[i]), float(en[i])) for i in range(n)]
+
+
+class AOSCCache:
+    """AOSCCache (reference sortformer.cpp:9-38): arrival-order speaker tracking.  A speaker arrives the first time its
+    probability is > 0.5 (fixed, not activity_threshold); within a frame speakers arrive in index order; a speaker is never
+    forgotten until reset()."""
+
+    def __init__(self, max_speakers: int = 4):
+        self.max_speakers = max_speakers
+        self.reset()
+
+    def update(self, probs: np.ndarray):
+        p = np.asarray(probs, np.float32)
+        for t in range(p.shape[0]):
+            for s in range(min(p.shape[1], self.max_speakers)):
+                if p[t, s] > np.float32(0.5) and not self._active[s]:
+                    self._active[s] = True
+                    self._order.append(s)
+
+    def speaker_order(self) -> List[int]:
+        return list(self._order)
+
+    def reset(self):
+        self._active = [False] * self.max_speakers
+        self._order = []
 
 
 # ------------------------------------------------------------------ result types (timestamp.hpp, transcribe.hpp)
@@ -715,6 +750,52 @@ class Engine:
 
     def fetch_probs(self, out: np.ndarray, lens: np.ndarray):
         self._check(self.L.pk_fetch_probs(self.h, _f32p(out), _i32p(lens)), "pk_fetch_probs")
+
+    # -- streaming diarization (a Sortformer engine): Sortformer::diarize_chunk for n_streams streams in lock step
+    def diar_stream_open(self, n_streams: int, max_chunk_samples: int = 16000, att_context_left: int = 70):
+        self._check(self.L.pk_diar_stream_open(self.h, n_streams, max_chunk_samples, att_context_left), "pk_diar_stream_open")
+        self.n_diar_streams = n_streams
+        self.diar_max_chunk = max_chunk_samples
+
+    def diar_stream_reset(self, stream: int = -1):
+        self._check(self.L.pk_diar_stream_reset(self.h, stream), "pk_diar_stream_reset")
+
+    def diar_stream_step(self, chunks: Sequence[np.ndarray], feats: bool = False, taps: bool = False):
+        """chunks[s] = stream s's input this step: 16 kHz PCM, or with feats=True its log-mel features [frames][mel_bins]
+        (an empty chunk = no input).  Returns (probs, frame_base): probs[s] the chunk-local activities [C_s][max_speakers]
+        of this step (C_s = 0 where the reference returns {}), frame_base[s] the absolute encoder frame of its first row;
+        with taps also the NEST encoder rows [C_s][d_model] per stream."""
+        S, SP = self.n_diar_streams, self.cfg.max_speakers
+        assert len(chunks) == S
+        nf_max = 1 + self.diar_max_chunk // 160
+        rows = S * (((7 + nf_max) // 8) * 8 // 8 + 1)
+        probs = np.zeros((rows, SP), np.float32)
+        n_out, base = np.zeros(S, np.int32), np.zeros(S, np.int32)
+        enc = np.zeros((rows, self.cfg.d_model), np.float32) if taps else None
+        encp = _f32p(enc) if taps else None
+        if feats:
+            fs = [np.asarray(f, np.float32).reshape(-1, self.cfg.mel_bins) for f in chunks]
+            nfr = np.array([f.shape[0] for f in fs], np.int32)
+            buf = np.ascontiguousarray(np.concatenate(fs, axis=0)) if nfr.sum() else np.zeros((1, self.cfg.mel_bins), np.float32)
+            st = self.L.pk_diar_stream_step_feats(self.h, _f32p(buf), _i32p(nfr), _f32p(probs), _i32p(n_out), _i32p(base), encp)
+            self._check(st, "pk_diar_stream_step_feats")
+        else:
+            buf, off = _pack(chunks)
+            self._check(self.L.pk_diar_stream_step(self.h, _f32p(buf), _i64p(off), _f32p(probs), _i32p(n_out), _i32p(base), encp),
+                        "pk_diar_stream_step")
+        o = np.concatenate([[0], np.cumsum(n_out)])
+        out = [probs[o[i]:o[i + 1]].copy() for i in range(S)]
+        if taps:
+            return out, base, [enc[o[i]:o[i + 1]].copy() for i in range(S)]
+        return out, base
+
+    def diar_stream_speakers(self, stream: int) -> List[int]:
+        """AOSCCache::speaker_order of one stream."""
+        order = np.zeros(max(self.cfg.max_speakers, 1), np.int32)
+        n = self.L.pk_diar_stream_speakers(self.h, stream, _i32p(order), len(order))
+        if n < 0:
+            raise RuntimeError("pk_diar_stream_speakers: invalid arguments")
+        return [int(v) for v in order[:n]]
 
     # -- phrase boosting on the device (SURVEY.md section 8f row 3)
     def set_boost(self, phrases: Sequence[Sequence[int]], boost: float = 5.0):
