@@ -14,7 +14,8 @@
 //   * the model only ever lives on the CUDA device: to_gpu() is a checked no-op and there
 //     is no CPU fallback;
 //   * transcribe_batch() is an addition (the reference is batch-1, transcribe.hpp:170-171);
-//   * phrase boosting (TranscribeOptions::boost_phrases) runs on the device for both decoders (pk_set_boost);
+//   * phrase boosting (TranscribeOptions::boost_phrases) runs on the device for both decoders (pk_set_boost); a batch may
+//     carry one TranscribeOptions per utterance (pk_set_boost_rows) and a stream its own phrases (pk_stream_set_boost);
 //   * TDTTranscriber passes blank = vocab-1 like the reference CLI (src/main.cpp:252), not
 //     the header's hard-coded 1024 (transcribe.hpp:256-261) which is wrong for 8193 tokens;
 //   * NemotronTranscriber decodes with blank = vocab-1 (8192) for the same reason: the reference's
@@ -251,6 +252,39 @@ inline std::vector<float> resample(const std::vector<float> &samples, int src_ra
 
 namespace detail {
 
+// A batch with one TranscribeOptions per utterance (transcribe_batch below).  The decoder and the timestamps flag belong to
+// the batch, so they must agree; an RNN-T model has no boosted decode (phrase_boost.hpp), so any phrase throws there.
+inline void check_batch_options(const std::vector<TranscribeOptions> &opts, size_t n_utts, bool rnnt_model) {
+    if (opts.size() != n_utts) throw std::invalid_argument("transcribe_batch: one TranscribeOptions per utterance expected");
+    for (const auto &o : opts) {
+        if (o.decoder != opts[0].decoder) throw std::invalid_argument("transcribe_batch: every utterance of a batch must name the same decoder");
+        if (o.timestamps != opts[0].timestamps) throw std::invalid_argument("transcribe_batch: timestamps must be the same for every utterance of a batch");
+        if (rnnt_model && !o.boost_phrases.empty())
+            throw std::runtime_error("RNNTTranscriber: phrase boosting covers CTC and TDT decodes only (phrase_boost.hpp)");
+    }
+}
+// The phrase lists of utterances [first, first + count) in the layout of pk_set_boost_rows: row i = phrases
+// [row[i], row[i+1]) of (ids, off), tokenised with ContextTrie::build as transcribe() does (phrases without tokens are skipped).
+struct BoostRows {
+    std::vector<int32_t> ids, off{0}, row{0};
+    std::vector<float> score;
+    bool any = false;
+};
+inline BoostRows pack_boost_rows(const std::vector<TranscribeOptions> &opts, size_t first, size_t count, const Tokenizer &tokenizer) {
+    BoostRows r;
+    for (size_t k = first; k < first + count; ++k) {
+        ContextTrie trie;
+        if (tokenizer.loaded()) trie.build(opts[k].boost_phrases, tokenizer);
+        const int32_t base = (int32_t)r.ids.size();
+        r.ids.insert(r.ids.end(), trie.ids().begin(), trie.ids().end());
+        for (size_t q = 1; q < trie.offsets().size(); ++q) r.off.push_back(base + trie.offsets()[q]);
+        r.row.push_back((int32_t)r.off.size() - 1);
+        r.score.push_back(opts[k].boost_score);
+        r.any |= !trie.empty();
+    }
+    return r;
+}
+
 class EngineHolder {
   public:
     EngineHolder(const pk_config &cfg, const std::string &weights, int device) : cfg_(cfg) {
@@ -344,6 +378,33 @@ class TranscriberBase {
             std::vector<size_t> n;
             for (size_t k = i; k < utts.size() && k < i + B; ++k) { p.push_back(utts[k].data()); n.push_back(utts[k].size()); }
             for (auto &toks : eng_->run(p, n, self().pick(decoder))) out.push_back(finish(toks, timestamps));
+        }
+        return out;
+    }
+    // One TranscribeOptions per utterance: every utterance is decoded with its own boost_phrases / boost_score, as
+    // transcribe() would decode it alone (pk_set_boost_rows); decoder and timestamps must agree across the batch.
+    std::vector<TranscribeResult> transcribe_batch(const std::vector<std::vector<float>> &utts, const std::vector<TranscribeOptions> &opts) {
+        check_batch_options(opts, utts.size(), eng_->cfg().n_durations == 0);
+        std::vector<TranscribeResult> out;
+        if (utts.empty()) return out;
+        struct RowsGuard {
+            pk_engine *e; bool on;
+            ~RowsGuard() { if (on) pk_set_boost_rows(e, nullptr, nullptr, nullptr, nullptr, 0); }
+        } guard{eng_->raw(), false};
+        const size_t B = (size_t)eng_->cfg().max_batch;
+        for (size_t i = 0; i < utts.size(); i += B) {
+            const size_t cnt = std::min(B, utts.size() - i);
+            const BoostRows r = pack_boost_rows(opts, i, cnt, tokenizer_);
+            if (r.any || guard.on) {
+                const int32_t none = 0;
+                if (pk_set_boost_rows(eng_->raw(), r.ids.empty() ? &none : r.ids.data(), r.off.data(), r.row.data(), r.score.data(), (int32_t)cnt) != PK_OK)
+                    throw std::runtime_error(std::string("parakeet_b200: ") + pk_last_error(eng_->raw()));
+                guard.on = true;
+            }
+            std::vector<const float *> p;
+            std::vector<size_t> n;
+            for (size_t k = i; k < i + cnt; ++k) { p.push_back(utts[k].data()); n.push_back(utts[k].size()); }
+            for (auto &toks : eng_->run(p, n, self().pick(opts[0].decoder))) out.push_back(finish(toks, opts[0].timestamps));
         }
         return out;
     }
@@ -543,6 +604,17 @@ class StreamingBatch {
         for (int s = 0; s < n_; ++s)
             if (stream < 0 || s == stream) { tokens_[s].clear(); stamped_[s].clear(); }
     }
+    /// The phrase list of ONE stream from its next step on (pk_stream_set_boost): its trie restarts at the root, its audio
+    /// state and tokens and every other stream are untouched; reset() keeps the list.  No phrases = not boosted.
+    void set_boost(int stream, const std::vector<std::string> &phrases, float boost_score = 5.0f) {
+        if (stream < 0 || stream >= n_) throw std::out_of_range("StreamingBatch::set_boost: no such stream");
+        ContextTrie trie;
+        if (tokenizer_.loaded()) trie.build(phrases, tokenizer_);
+        const int32_t none = 0;
+        if (pk_stream_set_boost(eng_->raw(), stream, trie.ids().empty() ? &none : trie.ids().data(), trie.offsets().data(),
+                                (int32_t)trie.offsets().size() - 1, boost_score) != PK_OK)
+            throw std::runtime_error(std::string("parakeet_b200: ") + pk_last_error(eng_->raw()));
+    }
     std::string get_text(int stream = 0) const { return (tokenizer_.loaded() && !tokens_[stream].empty()) ? tokenizer_.decode(tokens_[stream]) : std::string(); }
     const std::vector<TimestampedToken> &get_timestamped_tokens(int stream = 0) const { return stamped_[stream]; }
     const std::vector<int> &get_tokens(int stream = 0) const { return tokens_[stream]; }
@@ -597,6 +669,8 @@ class SingleStream {
         return transcribe_chunk(f.data(), f.size());
     }
     void reset() { batch_.reset(-1); }
+    /// Hot words of this stream from the next chunk on (TranscribeOptions::boost_phrases / boost_score for a stream).
+    void set_boost_phrases(const std::vector<std::string> &phrases, float boost_score = 5.0f) { batch_.set_boost(0, phrases, boost_score); }
     void set_partial_callback(PartialResultCallback cb) { cb_ = std::move(cb); }
     std::string get_text() const { return batch_.get_text(0); }
     const std::vector<TimestampedToken> &get_timestamped_tokens() const { return batch_.get_timestamped_tokens(0); }

@@ -340,6 +340,23 @@ typedef struct {
     int32_t grid, cl, upc, opc, out_in_smem, wih_in_smem, staged_ih, wstage_rows;
 } pk_tdt_hook_out;
 pk_status pk_kernel_tdt_decode(int device, const pk_tdt_hook_in *in, pk_tdt_hook_out *out, int64_t *guard_bad);
+/* The same launch with phrase boosting on and a phrase list and score per row, laid out as pk_set_boost_rows takes them
+ * (dec.n_dur > 0; n_utt rows).  With dec.carry the trie state on entry is trie_active0 [n_utt][64] / trie_nact0 [n_utt] (the
+ * bitmap follows from them); without, every row starts at the root.  Out: the decode's outputs plus the state on exit,
+ * trie_active [n_utt][64] (the first trie_nact[b] entries of a row are written), trie_nact [n_utt] and boost_bits
+ * [n_utt][(V + 31) / 32], all guarded. */
+typedef struct {
+    pk_tdt_hook_in dec;
+    const int32_t *phrase_ids, *phrase_off, *row_off;
+    const float *boost;                    /* [n_utt] */
+    const int32_t *trie_active0, *trie_nact0;
+} pk_tdt_boost_hook_in;
+typedef struct {
+    pk_tdt_hook_out dec;
+    int32_t *trie_active, *trie_nact;
+    uint32_t *boost_bits;
+} pk_tdt_boost_hook_out;
+pk_status pk_kernel_tdt_decode_boosted(int device, const pk_tdt_boost_hook_in *in, pk_tdt_boost_hook_out *out, int64_t *guard_bad);
 /* Streaming kernels as pk_stream_step launches them for one layer.  n_active of n_streams streams take part:
  * act_stream[a] is stream a's id, its rows are [row_off[a], row_off[a+1]) of the packed step (rows_total in all).
  * Per-stream state is indexed by stream id and updated in place; the updated state comes back in the *_out arrays.
@@ -397,10 +414,32 @@ int32_t pk_ctc_decode_boosted(const float *logprobs, int32_t n_frames, int32_t v
  * ContextTrie (:9-66) and keeps it on the device.  While set, every decode of this engine (pk_transcribe_batch,
  * pk_run_staged, pk_decode; CTC and TDT) adds `boost` to the label scores of the tokens that continue an active phrase;
  * the trie state is per utterance and advances on emissions; confidences stay exp(raw log-prob).  n_phrases = 0 clears
- * it.  (Not applied by pk_stream_step.)  At most 64 simultaneously active trie states per utterance.  The reference has
- * no boosted RNN-T decode: on an RNN-T model a non-empty phrase list is PK_ERR_INVALID.  pk_stream_open is also
- * PK_ERR_INVALID there (streaming decodes eou's TDT joint). */
+ * it.  This call gives every utterance the SAME list and score (and synchronises the engine stream); pk_set_boost_rows
+ * gives each utterance its own, pk_stream_set_boost each stream.  At most 64 simultaneously active trie states per
+ * utterance.  The reference has no boosted RNN-T decode: on an RNN-T model a non-empty phrase list is PK_ERR_INVALID.
+ * pk_stream_open is also PK_ERR_INVALID there (streaming decodes eou's TDT joint). */
 pk_status pk_set_boost(pk_engine *e, const int32_t *phrase_ids, const int32_t *phrase_off, int32_t n_phrases, float boost);
+/* Phrase lists per utterance, as TranscribeOptions::boost_phrases / boost_score belong to one transcribe() call of the
+ * reference (transcribe.hpp:38-43): for the following decodes (pk_transcribe_batch, pk_run_staged, pk_decode; CTC and TDT) row i
+ * of the batch uses phrases [row_off[i], row_off[i+1]) of (phrase_ids, phrase_off) with score boost[i], and decodes as the
+ * reference's *_boosted functions do on that utterance alone.  An empty range = that row decodes unboosted, bit for bit
+ * as with boosting off; rows >= n_rows of a later batch decode unboosted.  n_rows = 0 clears.  Replaces, and is replaced by,
+ * pk_set_boost.  Each row's trie lives in a slot of PK_BOOST_ROW_NODES nodes (root included): a longer list is
+ * PK_ERR_CAPACITY (the message names the row) and leaves the previous lists in force; n_rows > max_batch likewise.  The
+ * upload is ordered on the engine stream and does not synchronise, and changing lists re-captures no CUDA graph, so the call
+ * can be made for every batch of the pk_stage_pcm / pk_run_staged / pk_prefetch_pcm / pk_fetch_tokens pipeline.  RNN-T model
+ * with any phrase, Sortformer engine: PK_ERR_INVALID. */
+#define PK_BOOST_ROW_NODES 1024
+pk_status pk_set_boost_rows(pk_engine *e, const int32_t *phrase_ids, const int32_t *phrase_off, const int32_t *row_off,
+                            const float *boost, int32_t n_rows);
+/* The same for ONE open stream (0 <= stream < n_streams of pk_stream_open): takes effect from the next pk_stream_step, puts
+ * that stream's trie state back at the root, leaves its encoder caches / LSTM state / tokens and every other stream alone.
+ * n_phrases = 0 turns boosting off for the stream.  A boosted stream decodes as rnnt_streaming_decode_chunk (src/eou.cpp:17-98)
+ * with the label arg-max, trie advance and confidence of tdt_greedy_decode_with_timestamps_boosted (src/phrase_boost.cpp:266-352);
+ * the active trie states are carried from chunk to chunk (a phrase may straddle chunks) and pk_stream_reset returns them to
+ * the root, keeping the list (DESIGN.md section 8). */
+pk_status pk_stream_set_boost(pk_engine *e, int32_t stream, const int32_t *phrase_ids, const int32_t *phrase_off,
+                              int32_t n_phrases, float boost);
 
 /* Offline speaker diarization: Sortformer (include/parakeet/sortformer.hpp, src/sortformer.cpp:42-122 of the reference).
  * PCM -> log-mel WITHOUT per-bin normalisation (main.cpp:514-517) -> NEST encoder (the offline FastConformer under keys

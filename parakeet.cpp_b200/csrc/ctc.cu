@@ -55,16 +55,11 @@ ctc_frame_argmax_kernel(const float *__restrict__ logits, int M, int V, int ld, 
     }
 }
 
-// one warp per utterance; lane 0 scans (T' <= a few hundred frames)
-__global__ void ctc_collapse_kernel(const int32_t *__restrict__ best, const float *__restrict__ conf,
-                                    const int32_t *__restrict__ row_off, int n_utt, int blank, int cap,
-                                    int32_t *__restrict__ tok /* [n_utt][1+cap] */,
-                                    int32_t *__restrict__ t_start, int32_t *__restrict__ t_end,
-                                    float *__restrict__ t_conf) {
-    pdl_wait();
-    pdl_trigger();
-    const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= n_utt) return;
+// greedy collapse of utterance b from the per-frame arg-max, by one thread
+__device__ __forceinline__ void ctc_collapse_row(const int32_t *__restrict__ best, const float *__restrict__ conf,
+                                                 const int32_t *__restrict__ row_off, int b, int blank, int cap,
+                                                 int32_t *__restrict__ tok, int32_t *__restrict__ t_start,
+                                                 int32_t *__restrict__ t_end, float *__restrict__ t_conf) {
     const int r0 = row_off[b], T = row_off[b + 1] - r0;
     int32_t *ids = tok + (size_t)b * (1 + cap) + 1;
     int32_t *st = t_start + (size_t)b * cap, *en = t_end + (size_t)b * cap;
@@ -90,17 +85,29 @@ __global__ void ctc_collapse_kernel(const int32_t *__restrict__ best, const floa
     tok[(size_t)b * (1 + cap)] = n < cap ? n : cap;
 }
 
+// one thread per utterance scans (T' <= a few hundred frames)
+__global__ void ctc_collapse_kernel(const int32_t *__restrict__ best, const float *__restrict__ conf,
+                                    const int32_t *__restrict__ row_off, int n_utt, int blank, int cap,
+                                    int32_t *__restrict__ tok /* [n_utt][1+cap] */,
+                                    int32_t *__restrict__ t_start, int32_t *__restrict__ t_end,
+                                    float *__restrict__ t_conf) {
+    pdl_wait();
+    pdl_trigger();
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < n_utt) ctc_collapse_row(best, conf, row_off, b, blank, cap, tok, t_start, t_end, t_conf);
+}
+
 // ---- phrase-boosted CTC greedy decode (src/phrase_boost.cpp:70-176) ---------------------------------------------
 // One block per utterance walks the frames in order (the boosted token set depends on the tokens emitted so far): per
 // frame the block marks the children of the active trie states in a bitmap, takes argmax_v(logprob[v] + boost * [v
 // marked]) with the first maximum winning (strict '>' scan, :94-102), and thread 0 applies the CTC collapse rules and
 // advances the trie on an emission (:40-66: the root stays active, every state that continues with the token moves on).
-// Confidence = exp of the UNboosted log-prob (:110).
-constexpr int BOOST_MAX_ACTIVE = 64;
-
+// Confidence = exp of the UNboosted log-prob (:110).  Every utterance has its own trie and score (trie_row); one whose
+// trie is empty takes the plain collapse of the raw arg-max (best, conf), so it decodes exactly as without boosting.
 __global__ void __launch_bounds__(256)
-ctc_boosted_decode_kernel(const float *__restrict__ logprobs, const int32_t *__restrict__ row_off, int V, int blank, int cap,
-                          DeviceTrie trie, float boost, int32_t *__restrict__ tok, int32_t *__restrict__ t_start,
+ctc_boosted_decode_kernel(const float *__restrict__ logprobs, const int32_t *__restrict__ best, const float *__restrict__ conf,
+                          const int32_t *__restrict__ row_off, int V, int blank, int cap,
+                          DeviceTrie all_rows, int32_t *__restrict__ tok, int32_t *__restrict__ t_start,
                           int32_t *__restrict__ t_end, float *__restrict__ t_conf) {
     pdl_wait();
     pdl_trigger();
@@ -113,6 +120,12 @@ ctc_boosted_decode_kernel(const float *__restrict__ logprobs, const int32_t *__r
     __shared__ int red_i[8];
     __shared__ int s_nact, s_best;
     const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const TrieRow trie = trie_row(all_rows, b);
+    const float boost = trie.boost;
+    if (trie.empty()) {
+        if (tid == 0) ctc_collapse_row(best, conf, row_off, b, blank, cap, tok, t_start, t_end, t_conf);
+        return;
+    }
     const int r0 = row_off[b], T = row_off[b + 1] - r0;
     int32_t *ids = tok + (size_t)b * (1 + cap) + 1;
     int32_t *st = t_start + (size_t)b * cap, *en = t_end + (size_t)b * cap;
@@ -207,11 +220,11 @@ ctc_boosted_decode_kernel(const float *__restrict__ logprobs, const int32_t *__r
 
 }  // namespace
 
-void launch_ctc_boosted_decode(const float *logprobs, const int32_t *row_off, int n_utt, int V, int blank, int cap,
-                               const DeviceTrie &trie, float boost, int32_t *tok, int32_t *t_start, int32_t *t_end, float *t_conf,
+void launch_ctc_boosted_decode(const float *logprobs, const int32_t *best, const float *conf, const int32_t *row_off, int n_utt, int V, int blank, int cap,
+                               const DeviceTrie &trie, int32_t *tok, int32_t *t_start, int32_t *t_end, float *t_conf,
                                cudaStream_t st) {
     const size_t smem = sizeof(uint32_t) * ((V + 31) / 32) + sizeof(int) * 2 * BOOST_MAX_ACTIVE;
-    launch_pdl(ctc_boosted_decode_kernel, dim3(n_utt), dim3(256), smem, st, logprobs, row_off, V, blank, cap, trie, boost, tok, t_start, t_end, t_conf);
+    launch_pdl(ctc_boosted_decode_kernel, dim3(n_utt), dim3(256), smem, st, logprobs, best, conf, row_off, V, blank, cap, trie, tok, t_start, t_end, t_conf);
 }
 
 void launch_ctc_frame_argmax(const float *logits, int M, int V, int ld, int32_t *best, float *conf,

@@ -774,7 +774,7 @@ pk_status pk_engine::run_ctc(float *logprobs_dev) {
     ep.out_f32 = logits;
     ep.ldo = ldv;
     gemm(enc_operand(this), c.d_model, ctc_head, M, ep);
-    if (boost_on && !logprobs_dev) {
+    if (boosting() && !logprobs_dev) {
         // boosted decode compares log-probs + boost (phrase_boost.cpp:94-102): they land in the (idle) qkv workspace
         if ((size_t)M * c.vocab > (size_t)Bmax * Tmax * 3 * c.d_model) return fail(PK_ERR_CAPACITY, "boosted CTC decode: workspace too small for the log-probs");
         logprobs_dev = qkv;
@@ -782,8 +782,8 @@ pk_status pk_engine::run_ctc(float *logprobs_dev) {
     {
         Scope sc(this, CAT_CTC);
         launch_ctc_frame_argmax(logits, M, c.vocab, ldv, best, bconf, logprobs_dev, stream);
-        if (boost_on)
-            launch_ctc_boosted_decode(logprobs_dev, d_row_off, n_utt, c.vocab, c.vocab - 1, cap, trie, boost, tok, t_start, t_end, t_conf, stream);
+        if (boosting())
+            launch_ctc_boosted_decode(logprobs_dev, best, bconf, d_row_off, n_utt, c.vocab, c.vocab - 1, cap, boost_trie(), tok, t_start, t_end, t_conf, stream);
         else
             launch_ctc_collapse(best, bconf, d_row_off, n_utt, c.vocab - 1, cap, tok, t_start, t_end, t_conf, stream);
     }
@@ -817,7 +817,7 @@ pk_status pk_engine::run_tdt() {
     p.key_lab = tdt_keys; p.key_dur = tdt_keys + 3 * (size_t)Bpad;
     p.dbg = reinterpret_cast<long long *>(tdt_keys + 6 * (size_t)Bpad);
     p.tok = tok; p.t_start = t_start; p.t_end = t_end; p.t_conf = t_conf;
-    p.boost_on = boost_on ? 1 : 0; p.boost = boost; p.trie = trie; p.boost_bits = boost_bits; p.trie_active = trie_active; p.trie_nact = trie_nact;
+    p.boost_on = boosting() ? 1 : 0; p.trie = boost_trie(); p.boost_bits = boost_bits; p.trie_active = trie_active; p.trie_nact = trie_nact;
     // initial state: zero LSTM state, token = blank (SOS), t = 0 (tdt.cpp:49-59)
     const size_t HS = (size_t)p.P * bp;
     PK_CUDA(cudaMemsetAsync(hbuf, 0, HS * 2 * p.L * sizeof(float), stream));
@@ -1143,6 +1143,10 @@ void pk_engine_destroy(pk_engine *e) {
     if (e->h_te) cudaFreeHost(e->h_te);
     if (e->h_tc) cudaFreeHost(e->h_tc);
     if (e->h_probs) cudaFreeHost(e->h_probs);
+    for (int i = 0; i < 2; ++i) {
+        if (e->h_bstage[i]) cudaFreeHost(e->h_bstage[i]);
+        if (e->ev_bstage[i]) cudaEventDestroy(e->ev_bstage[i]);
+    }
     if (e->ev_h2d) cudaEventDestroy(e->ev_h2d);
     if (e->ev_front) cudaEventDestroy(e->ev_front);
     for (int i = 0; i < pk_engine::H2D_CHUNKS; ++i)
@@ -1710,7 +1714,8 @@ pk_status pk_run_staged(pk_engine *e, pk_decoder dec) {
         if (fs) return fs;
     }
     std::string key(1, dec == PK_DECODER_CTC ? 'c' : (dec == PK_DECODER_RNNT ? 'r' : 't'));
-    const int32_t bg = e->boost_on ? e->boost_gen : 0;
+    // (per-row lists live in buffers that never move: one graph serves every set of lists)
+    const int32_t bg = e->brows_on ? -1 : (e->boost_on ? e->boost_gen : 0);
     key.append(reinterpret_cast<const char *>(&bg), sizeof(bg));
     key.append(reinterpret_cast<const char *>(e->frame_off.data()), e->frame_off.size() * sizeof(int32_t));
     return e->run_graphed(key, [e, dec]() { return run_pipeline(e, dec); });
@@ -1971,6 +1976,57 @@ pk_status pk_resample_batch(pk_engine *e, const float *pcm, const int64_t *offse
 // ===================================================================== phrase boosting (SURVEY.md section 8f row 3)
 // ContextTrie (src/phrase_boost.cpp:9-66) built on the host from token-id phrases, flattened to CSR (children of a node
 // sorted by token) and uploaded; the decode kernels (ctc.cu: ctc_boosted_decode_kernel, tdt.cu: boost_on) walk it.
+pk_status pk_engine::boost_state_alloc() {
+    if (boost_bits) return PK_OK;
+    const size_t W = ((size_t)cfg.vocab + 31) / 32;
+    boost_bits = dalloc<uint32_t>((size_t)Bpad * W);
+    trie_active = dalloc<int32_t>((size_t)Bpad * BOOST_MAX_ACTIVE);
+    trie_nact = dalloc<int32_t>(Bpad);
+    if (!boost_bits || !trie_active || !trie_nact) return fail(PK_ERR_CUDA, "cudaMalloc failed (boost state)");
+    // the decode reads the bitmaps of the padding rows [n_utt, Bpad) too, and no launch ever writes those: they stay zero
+    PK_CUDA(cudaMemsetAsync(boost_bits, 0, (size_t)Bpad * W * sizeof(uint32_t), stream));
+    return PK_OK;
+}
+
+pk_status pk_engine::boost_upload(const char *fn, BoostSlots &dst, int row0, int n, int n_clear, const int32_t *phrase_ids,
+                                  const int32_t *phrase_off, const int32_t *row_off, const float *boost, bool *any) {
+    const int rows = n + n_clear;
+    if (rows <= 0) return PK_OK;
+    if (rows > Bmax) return fail(PK_ERR_CAPACITY, std::string(fn) + ": more rows than pk_config.max_batch");
+    for (int k = 0; k < 2; ++k)                        // first use (a buffer or event that exists is kept: a failed attempt leaks nothing)
+        if ((!ev_bstage[k] && cudaEventCreateWithFlags(&ev_bstage[k], cudaEventDisableTiming) != cudaSuccess) ||
+            (!h_bstage[k] && cudaMallocHost(&h_bstage[k], (size_t)Bmax * (BOOST_SLOT_INTS + 1) * sizeof(int32_t)) != cudaSuccess))
+            return fail(PK_ERR_CUDA, "cudaMallocHost failed (boost staging)");
+    bstage_rows = Bmax;
+    const int k = bstage_next;
+    cudaEventSynchronize(ev_bstage[k]);                // the upload before last has left this buffer (normally long ago)
+    int32_t *hs = h_bstage[k];
+    float *hv = reinterpret_cast<float *>(hs + (size_t)bstage_rows * BOOST_SLOT_INTS);
+    std::vector<int32_t> first, tk, cd;
+    *any = false;
+    for (int i = 0; i < rows; ++i) {
+        int32_t *slot = hs + (size_t)i * BOOST_SLOT_INTS;
+        slot[0] = slot[1] = 0;                         // an empty slot: the row is not boosted
+        hv[i] = 0.f;
+        if (i >= n || row_off[i + 1] == row_off[i]) continue;
+        if (!boost_trie_csr(phrase_ids, phrase_off, row_off[i], row_off[i + 1], first, tk, cd))
+            return fail(PK_ERR_INVALID, std::string(fn) + ": phrase_off must be non-decreasing");
+        if ((int)first.size() - 1 > BOOST_SLOT_NODES)
+            return fail(PK_ERR_CAPACITY, std::string(fn) + ": the phrases of row " + std::to_string(row0 + i) + " make a trie of " +
+                                             std::to_string(first.size() - 1) + " nodes; a row holds at most " + std::to_string(BOOST_SLOT_NODES));
+        memcpy(slot, first.data(), first.size() * sizeof(int32_t));
+        memcpy(slot + BOOST_SLOT_NODES + 1, tk.data(), tk.size() * sizeof(int32_t));
+        memcpy(slot + BOOST_SLOT_NODES + 1 + BOOST_SLOT_EDGES, cd.data(), cd.size() * sizeof(int32_t));
+        hv[i] = boost[i];
+        *any |= !tk.empty();
+    }
+    PK_CUDA(cudaMemcpyAsync(dst.slots + (size_t)row0 * BOOST_SLOT_INTS, hs, (size_t)rows * BOOST_SLOT_INTS * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+    PK_CUDA(cudaMemcpyAsync(dst.val + row0, hv, (size_t)rows * sizeof(float), cudaMemcpyHostToDevice, stream));
+    PK_CUDA(cudaEventRecord(ev_bstage[k], stream));
+    bstage_next = 1 - k;
+    return PK_OK;
+}
+
 pk_status pk_set_boost(pk_engine *e, const int32_t *phrase_ids, const int32_t *phrase_off, int32_t n_phrases, float boost) {
     if (!e || n_phrases < 0 || (n_phrases > 0 && (!phrase_ids || !phrase_off))) return PK_ERR_INVALID;
     if (e->diar) return e->fail(PK_ERR_INVALID, "pk_set_boost: a Sortformer engine has no decoder");
@@ -1979,50 +2035,60 @@ pk_status pk_set_boost(pk_engine *e, const int32_t *phrase_ids, const int32_t *p
     cudaSetDevice(e->device);
     cudaStreamSynchronize(e->stream);
     ++e->boost_gen;
+    e->brows_on = false;
     if (n_phrases == 0) {
         e->boost_on = false;
         return PK_OK;
     }
-    std::vector<std::map<int32_t, int32_t>> ch(1);
-    for (int32_t p = 0; p < n_phrases; ++p) {
-        int32_t node = 0;
-        if (phrase_off[p + 1] < phrase_off[p]) return e->fail(PK_ERR_INVALID, "pk_set_boost: phrase_off must be non-decreasing");
-        for (int32_t i = phrase_off[p]; i < phrase_off[p + 1]; ++i) {
-            auto it = ch[node].find(phrase_ids[i]);
-            if (it == ch[node].end()) {
-                const int32_t nx = (int32_t)ch.size();
-                ch[node][phrase_ids[i]] = nx;
-                ch.emplace_back();
-                node = nx;
-            } else {
-                node = it->second;
-            }
-        }
-    }
-    std::vector<int32_t> first(ch.size() + 1, 0), tk, cd;
-    for (size_t i = 0; i < ch.size(); ++i) {
-        for (auto &kv : ch[i]) {
-            tk.push_back(kv.first);
-            cd.push_back(kv.second);
-        }
-        first[i + 1] = (int32_t)tk.size();
-    }
+    std::vector<int32_t> first, tk, cd;
+    if (!boost_trie_csr(phrase_ids, phrase_off, 0, n_phrases, first, tk, cd)) return e->fail(PK_ERR_INVALID, "pk_set_boost: phrase_off must be non-decreasing");
     if (tk.empty()) {       // only empty phrases
         e->boost_on = false;
         return PK_OK;
     }
     int32_t *d_first = e->upload(first), *d_tok = e->upload(tk), *d_child = e->upload(cd);
     if (!d_first || !d_tok || !d_child) return e->fail(PK_ERR_CUDA, "cudaMalloc failed (trie)");
-    e->trie.first = d_first; e->trie.tok = d_tok; e->trie.child = d_child; e->trie.n_nodes = (int32_t)ch.size();
-    if (!e->boost_bits) {
-        const size_t W = ((size_t)e->cfg.vocab + 31) / 32;
-        e->boost_bits = e->dalloc<uint32_t>((size_t)e->Bpad * W);
-        e->trie_active = e->dalloc<int32_t>((size_t)e->Bpad * 64);
-        e->trie_nact = e->dalloc<int32_t>(e->Bpad);
-        if (!e->boost_bits || !e->trie_active || !e->trie_nact) return e->fail(PK_ERR_CUDA, "cudaMalloc failed (boost state)");
-    }
-    e->boost = boost;
+    e->trie = DeviceTrie{};
+    e->trie.first = d_first; e->trie.tok = d_tok; e->trie.child = d_child; e->trie.n_nodes = (int32_t)first.size() - 1;
+    e->trie.boost = boost;
+    if (pk_status s = e->boost_state_alloc()) return s;
     e->boost_on = true;
+    return PK_OK;
+}
+
+pk_status pk_set_boost_rows(pk_engine *e, const int32_t *phrase_ids, const int32_t *phrase_off, const int32_t *row_off, const float *boost,
+                            int32_t n_rows) {
+    if (!e || n_rows < 0 || (n_rows > 0 && (!row_off || !boost))) return PK_ERR_INVALID;
+    if (e->diar) return e->fail(PK_ERR_INVALID, "pk_set_boost_rows: a Sortformer engine has no decoder");
+    if (n_rows > e->Bmax) return e->fail(PK_ERR_CAPACITY, "pk_set_boost_rows: more rows than pk_config.max_batch");
+    for (int32_t i = 0; i < n_rows; ++i)
+        if (row_off[i + 1] < row_off[i] || row_off[i] < 0) return e->fail(PK_ERR_INVALID, "pk_set_boost_rows: row_off must be non-decreasing");
+    const bool lists = n_rows > 0 && row_off[n_rows] > row_off[0];
+    if (lists && (!phrase_ids || !phrase_off)) return PK_ERR_INVALID;
+    if (e->cfg.n_durations == 0 && lists)
+        return e->fail(PK_ERR_INVALID, "pk_set_boost_rows: phrase boosting covers CTC and TDT decodes; this is an RNN-T model");
+    cudaSetDevice(e->device);
+    if (!lists && !e->brows.slots) {                   // nothing to boost and nothing on the device to clear
+        e->boost_on = e->brows_on = false;
+        return PK_OK;
+    }
+    if (!e->brows.slots) {
+        e->brows.slots = e->dalloc<int32_t>((size_t)e->Bmax * BOOST_SLOT_INTS);
+        e->brows.val = e->dalloc<float>(e->Bmax);
+        e->brows.rows = e->Bmax;
+        if (!e->brows.slots || !e->brows.val) return e->fail(PK_ERR_CUDA, "cudaMalloc failed (boost slots)");
+        // every slot starts empty (first[0] == first[1]): a row no call has named decodes unboosted
+        if (cudaMemsetAsync(e->brows.slots, 0, (size_t)e->Bmax * BOOST_SLOT_INTS * sizeof(int32_t), e->stream) != cudaSuccess ||
+            cudaMemsetAsync(e->brows.val, 0, (size_t)e->Bmax * sizeof(float), e->stream) != cudaSuccess)
+            return e->fail(PK_ERR_CUDA, "cudaMemset failed (boost slots)");
+    }
+    if (pk_status s = e->boost_state_alloc()) return s;
+    bool any = false;
+    const int n_clear = std::max(0, e->brows_hi - n_rows);   // rows of an earlier call that this one does not name
+    if (pk_status s = e->boost_upload("pk_set_boost_rows", e->brows, 0, n_rows, n_clear, phrase_ids, phrase_off, row_off, boost, &any)) return s;
+    e->brows_hi = n_rows;
+    e->boost_on = false;
+    e->brows_on = any;
     return PK_OK;
 }
 

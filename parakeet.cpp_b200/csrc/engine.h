@@ -72,6 +72,8 @@ struct TLayerW {
     float *n1_w, *n1_b, *n2_w, *n2_b;
 };
 
+static_assert(BOOST_SLOT_NODES == PK_BOOST_ROW_NODES, "the slot capacity is part of the C-ABI");
+
 }  // namespace pk_detail
 using namespace pk_detail;
 
@@ -188,13 +190,28 @@ struct pk_engine {
     bool last_tdt = false;                             // the token buffer holds a TDT decode (overflow flags are valid)
     int32_t truncated = 0;                             // utterances of the last fetch whose TDT hypothesis hit the token capacity
 
-    // ---- phrase boosting (pk_set_boost): ContextTrie on the device + per-utterance trie state of the TDT kernel
-    DeviceTrie trie{};
+    // ---- phrase boosting: ContextTrie on the device + per-utterance trie state of the TDT kernel
+    DeviceTrie trie{};                                 // pk_set_boost: one trie and score for every utterance
     bool boost_on = false;
-    float boost = 0.f;
     int boost_gen = 0;                                 // bumps on every pk_set_boost (part of the CUDA-graph key)
     uint32_t *boost_bits = nullptr;                    // [Bpad][(V+31)/32]
     int32_t *trie_active = nullptr, *trie_nact = nullptr;
+    BoostSlots brows;                                  // pk_set_boost_rows: a trie and score per utterance of the batch
+    bool brows_on = false;                             // some row of brows has a list (replaces, and is replaced by, boost_on)
+    int brows_hi = 0;                                  // rows [0, brows_hi) of brows may hold a list on the device
+    // List uploads go through two pinned buffers used in turn ([rows][BOOST_SLOT_INTS] ints, then [rows] scores), so an
+    // upload never waits for the stream unless two earlier ones are still queued.
+    int32_t *h_bstage[2] = {};
+    cudaEvent_t ev_bstage[2] = {};
+    int bstage_rows = 0, bstage_next = 0;
+    pk_status boost_state_alloc();                     // boost_bits / trie_active / trie_nact
+    // Rows [row0, row0 + n) of `dst` <- the tries of lists i = phrases [row_off[i], row_off[i+1]) with scores boost[i]; the
+    // n_clear rows after them <- empty.  Stream-ordered, no synchronisation.  Nothing is uploaded when a list is invalid
+    // or over the slot capacity (PK_ERR_CAPACITY naming the row).  *any: some list has an edge.
+    pk_status boost_upload(const char *fn, BoostSlots &dst, int row0, int n, int n_clear, const int32_t *phrase_ids,
+                           const int32_t *phrase_off, const int32_t *row_off, const float *boost, bool *any);
+    bool boosting() const { return boost_on || brows_on; }
+    DeviceTrie boost_trie() const { return brows_on ? brows.trie() : trie; }
 
     // ---- optional per-kernel-class timing (CUDA events on the engine stream)
     enum { CAT_MEL, CAT_SUBSAMPLE, CAT_GEMM, CAT_LAYERNORM, CAT_ATTENTION, CAT_DWCONV, CAT_CTC, CAT_TDT, CAT_MHA, CAT_HEAD, CAT_N };

@@ -325,7 +325,9 @@ pk_status pk_kernel_ctc_argmax(int device, int M, int V, int ld, const float *lo
     return PK_OK;
 }
 
-pk_status pk_kernel_tdt_decode(int device, const pk_tdt_hook_in *in, pk_tdt_hook_out *out, int64_t *guard_bad) {
+// bin / bout: the boosted form (pk_kernel_tdt_decode_boosted), else null
+static pk_status tdt_hook_run(int device, const pk_tdt_hook_in *in, pk_tdt_hook_out *out, int64_t *guard_bad, const pk_tdt_boost_hook_in *bin,
+                              pk_tdt_boost_hook_out *bout) {
     if (!in || !out) return PK_ERR_INVALID;
     const int P = in->P, J = in->J, V = in->V, D = in->n_dur, L = in->L, n = in->n_utt;
     if (P < 32 || P % 32 || J < 32 || J % 32 || V < 2 || D < 0 || D > 8 || L < 1 || L > PK_MAX_LSTM || n < 1 || in->cap < 1 ||
@@ -405,6 +407,56 @@ pk_status pk_kernel_tdt_decode(int device, const pk_tdt_hook_in *in, pk_tdt_hook
             cudaMemcpy(p.tok_state, in->tok0, (size_t)n * 4, cudaMemcpyHostToDevice) != cudaSuccess)
             return PK_ERR_CUDA;
     }
+    const int BW = (V + 31) / 32;
+    if (bin) {
+        // one trie slot per row, as pk_set_boost_rows lays them out; the state on entry: the root, or the caller's active sets
+        if (D == 0 || !bin->row_off || !bin->boost || (in->carry && (!bin->trie_active0 || !bin->trie_nact0))) return PK_ERR_INVALID;
+        std::vector<int32_t> slots((size_t)n * BOOST_SLOT_INTS, 0), act((size_t)n * BOOST_MAX_ACTIVE, 0), nact(n, 1), first, tk, cd;
+        std::vector<uint32_t> bits((size_t)n * BW, 0u);
+        for (int b = 0; b < n; ++b) {
+            int32_t *slot = &slots[(size_t)b * BOOST_SLOT_INTS], *tok = slot + BOOST_SLOT_NODES + 1, *child = tok + BOOST_SLOT_EDGES;
+            if (bin->row_off[b + 1] < bin->row_off[b]) return PK_ERR_INVALID;
+            if (bin->row_off[b + 1] > bin->row_off[b]) {
+                if (!bin->phrase_ids || !bin->phrase_off || !boost_trie_csr(bin->phrase_ids, bin->phrase_off, bin->row_off[b], bin->row_off[b + 1], first, tk, cd))
+                    return PK_ERR_INVALID;
+                if ((int)first.size() - 1 > BOOST_SLOT_NODES) return PK_ERR_CAPACITY;
+                memcpy(slot, first.data(), first.size() * 4);
+                memcpy(tok, tk.data(), tk.size() * 4);
+                memcpy(child, cd.data(), cd.size() * 4);
+            }
+            if (in->carry) {
+                nact[b] = bin->trie_nact0[b];
+                if (nact[b] < 1 || nact[b] > BOOST_MAX_ACTIVE) return PK_ERR_INVALID;
+                memcpy(&act[(size_t)b * BOOST_MAX_ACTIVE], bin->trie_active0 + (size_t)b * BOOST_MAX_ACTIVE, (size_t)nact[b] * 4);
+            }
+            const int n_nodes = slot[0] == slot[1] ? 1 : (int)first.size() - 1;
+            for (int a = 0; a < nact[b]; ++a) {
+                const int node = act[(size_t)b * BOOST_MAX_ACTIVE + a];
+                if (node < 0 || node >= n_nodes) return PK_ERR_INVALID;
+                for (int e = slot[node]; e < slot[node + 1]; ++e)
+                    if (tok[e] >= 0 && tok[e] < V) bits[(size_t)b * BW + (tok[e] >> 5)] |= 1u << (tok[e] & 31);
+            }
+        }
+        BoostSlots bs;
+        bs.slots = cx.upload(slots.data(), slots.size());
+        bs.val = cx.upload(bin->boost, n);
+        p.boost_on = 1;
+        p.trie = bs.trie();
+        // (the decode reads the bitmaps of all Bpad rows: the padding rows read zeros)
+        p.boost_bits = cx.guarded<uint32_t>((size_t)Bpad * BW);
+        p.trie_active = cx.guarded<int32_t>((size_t)n * BOOST_MAX_ACTIVE);
+        p.trie_nact = cx.guarded<int32_t>(n);
+        if (!cx.ok || cudaMemset(p.boost_bits, 0, (size_t)Bpad * BW * 4) != cudaSuccess) return PK_ERR_CUDA;
+        if (in->carry) {
+            // entries past a row's active set stay 0xFF: the kernel must not read them
+            for (int b = 0; b < n; ++b)
+                if (cudaMemcpy(p.trie_active + (size_t)b * BOOST_MAX_ACTIVE, &act[(size_t)b * BOOST_MAX_ACTIVE], (size_t)nact[b] * 4, cudaMemcpyHostToDevice) != cudaSuccess)
+                    return PK_ERR_CUDA;
+            if (cudaMemcpy(p.trie_nact, nact.data(), (size_t)n * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
+                cudaMemcpy(p.boost_bits, bits.data(), bits.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess)
+                return PK_ERR_CUDA;
+        }
+    }
     if (!cx.ok || !cx.sync()) return PK_ERR_CUDA;
     int sms = 0;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
@@ -479,7 +531,19 @@ pk_status pk_kernel_tdt_decode(int device, const pk_tdt_hook_in *in, pk_tdt_hook
         if (out->c_state)
             for (int l = 0; l < L; ++l) memcpy(out->c_state + (size_t)l * n * P, &c[(size_t)l * Bpad * P], (size_t)n * P * 4);
     }
+    if (bout && (!fetch_i32(bout->trie_active, p.trie_active, (size_t)n * BOOST_MAX_ACTIVE) || !fetch_i32(bout->trie_nact, p.trie_nact, n) ||
+                 !fetch_i32(reinterpret_cast<int32_t *>(bout->boost_bits), reinterpret_cast<const int32_t *>(p.boost_bits), (size_t)n * BW)))
+        return PK_ERR_CUDA;
     return PK_OK;
+}
+
+pk_status pk_kernel_tdt_decode(int device, const pk_tdt_hook_in *in, pk_tdt_hook_out *out, int64_t *guard_bad) {
+    return tdt_hook_run(device, in, out, guard_bad, nullptr, nullptr);
+}
+
+pk_status pk_kernel_tdt_decode_boosted(int device, const pk_tdt_boost_hook_in *in, pk_tdt_boost_hook_out *out, int64_t *guard_bad) {
+    if (!in || !out) return PK_ERR_INVALID;
+    return tdt_hook_run(device, &in->dec, &out->dec, guard_bad, in, out);
 }
 
 }  // extern "C"

@@ -32,6 +32,13 @@ struct StreamSet {
     float *c_state = nullptr;                                  // [lstm][Bpad][P]
     float *hbuf = nullptr;                                     // bf16 planes [hi|lo][lstm][2][Bpad][P]
     int32_t *tok_state = nullptr;
+    // Phrase boosting per stream (pk_stream_set_boost): a trie slot and score per stream, and the trie state of the decode
+    // kernel, carried from chunk to chunk like the LSTM state.
+    BoostSlots boost;
+    uint32_t *boost_bits = nullptr;                            // [Bpad][(V+31)/32]
+    int32_t *trie_active = nullptr, *trie_nact = nullptr;      // [Bpad][64], [Bpad]
+    std::vector<uint8_t> boosted;                              // stream has a list
+    int n_boosted = 0;
     // per-step device scratch
     float *d_chunk = nullptr, *ssig = nullptr, *mel_in = nullptr;
     StreamPlan *d_plan = nullptr, *h_plan = nullptr;           // h_plan pinned
@@ -170,6 +177,7 @@ pk_status pk_engine::run_stream_decode() {
     p.dbg = reinterpret_cast<long long *>(tdt_keys + 6 * (size_t)Bpad);
     p.tok = tok; p.t_start = t_start; p.t_end = t_end; p.t_conf = t_conf;
     p.carry = 1; p.c_state = s.c_state; p.tok_state = s.tok_state; p.frame_base = s.d_meta + 5 * s.S;
+    p.boost_on = s.n_boosted > 0 ? 1 : 0; p.trie = s.boost.trie(); p.boost_bits = s.boost_bits; p.trie_active = s.trie_active; p.trie_nact = s.trie_nact;
     cudaError_t ce;
     {
         Scope sc(this, CAT_TDT);
@@ -211,14 +219,26 @@ pk_status pk_stream_open(pk_engine *e, int32_t n_streams, int32_t max_chunk_samp
     s->c_state = e->dalloc<float>((size_t)LL * e->Bpad * P);
     s->hbuf = e->dalloc<float>((size_t)P * e->Bpad * 2 * LL);
     s->tok_state = e->dalloc<int32_t>(e->Bpad);
+    s->boost.slots = e->dalloc<int32_t>((size_t)S * BOOST_SLOT_INTS);
+    s->boost.val = e->dalloc<float>(S);
+    s->boost.rows = S;
+    s->boost_bits = e->dalloc<uint32_t>((size_t)e->Bpad * ((c.vocab + 31) / 32));
+    s->trie_active = e->dalloc<int32_t>((size_t)e->Bpad * BOOST_MAX_ACTIVE);
+    s->trie_nact = e->dalloc<int32_t>(e->Bpad);
+    s->boosted.assign(S, 0);
     s->d_chunk = e->dalloc<float>((size_t)S * max_chunk_samples + 8);
     s->ssig = e->dalloc<float>((size_t)S * (max_chunk_samples + STREAM_OVL_CAP) + 8);
     s->mel_in = e->dalloc<float>((size_t)S * (8 + s->nf_max) * c.mel_bins);
     s->d_plan = e->dalloc<StreamPlan>(S);
     s->d_sig_off = e->dalloc<int64_t>(S + 1);
     s->d_meta = e->dalloc<int32_t>((size_t)7 * S + 8);
-    if (!s->d_meta || !s->d_plan || !s->mel_in || !s->ssig || !s->kc || !s->vc || !s->convc || !s->hbuf)
+    if (!s->d_meta || !s->d_plan || !s->mel_in || !s->ssig || !s->kc || !s->vc || !s->convc || !s->hbuf || !s->boost.slots || !s->boost.val ||
+        !s->boost_bits || !s->trie_active || !s->trie_nact)
         return e->fail(PK_ERR_CUDA, "cudaMalloc failed (stream state)");
+    // every slot empty (first[0] == first[1]): no stream is boosted until pk_stream_set_boost
+    if (cudaMemsetAsync(s->boost.slots, 0, (size_t)S * BOOST_SLOT_INTS * sizeof(int32_t), e->stream) != cudaSuccess ||
+        cudaMemsetAsync(s->boost_bits, 0, (size_t)e->Bpad * ((c.vocab + 31) / 32) * sizeof(uint32_t), e->stream) != cudaSuccess)
+        return e->fail(PK_ERR_CUDA, "cudaMemset failed (stream boost state)");
     if (cudaMallocHost(&s->h_plan, sizeof(StreamPlan) * S) != cudaSuccess || cudaMallocHost(&s->h_sig_off, sizeof(int64_t) * (S + 1)) != cudaSuccess ||
         cudaMallocHost(&s->h_meta, sizeof(int32_t) * (7 * S + 8)) != cudaSuccess ||
         cudaMallocHost(&s->h_chunk, sizeof(float) * ((size_t)S * max_chunk_samples + 8)) != cudaSuccess ||
@@ -256,6 +276,11 @@ pk_status pk_stream_reset(pk_engine *e, int32_t stream) {
                 if (ce == cudaSuccess) ce = cudaMemsetAsync(hb + lo + (size_t)(l * 2 + pl) * HS + (size_t)i * P, 0, sizeof(bf16) * P, e->stream);
             }
         }
+    }
+    // the phrase trie restarts at the root (the stream keeps its list)
+    if (ce == cudaSuccess) {
+        launch_boost_state_reset(s.boost.trie(), c.vocab, s0, s1 - s0, s.boost_bits, s.trie_active, s.trie_nact, e->stream);
+        ce = cudaGetLastError();
     }
     if (ce == cudaSuccess) {
         std::vector<int32_t> blank(s1 - s0, c.vocab - 1);
@@ -381,7 +406,8 @@ pk_status pk_stream_step(pk_engine *e, const float *pcm, const int64_t *offsets,
             ps = body();                       // (debug taps: plain launches)
         } else {
             // every kernel argument of the step depends only on which streams take how many frames: one graph per pattern
-            std::string key(1, 's');
+            // (and on whether any stream is boosted: the lists themselves live in buffers that never move)
+            std::string key(1, s.n_boosted > 0 ? 'b' : 's');
             key.append(reinterpret_cast<const char *>(s.act.data()), s.act.size() * sizeof(int32_t));
             key.append(reinterpret_cast<const char *>(s.take.data()), s.take.size() * sizeof(int32_t));
             ps = e->run_graphed(key, body);
@@ -397,6 +423,24 @@ pk_status pk_stream_step(pk_engine *e, const float *pcm, const int64_t *offsets,
     }
     e->n_utt = S;                                   // the token rows cover all streams
     return e->fetch(out);
+}
+
+pk_status pk_stream_set_boost(pk_engine *e, int32_t stream, const int32_t *phrase_ids, const int32_t *phrase_off, int32_t n_phrases, float boost) {
+    if (!e || n_phrases < 0 || (n_phrases > 0 && (!phrase_ids || !phrase_off))) return PK_ERR_INVALID;
+    cudaSetDevice(e->device);
+    if (e->diar) return e->fail(PK_ERR_INVALID, "pk_stream_set_boost: a Sortformer engine has no decoder");
+    if (!e->ss) return e->fail(PK_ERR_INVALID, "pk_stream_set_boost: no streams are open (pk_stream_open)");
+    StreamSet &s = *e->ss;
+    if (stream < 0 || stream >= s.S) return e->fail(PK_ERR_INVALID, "pk_stream_set_boost: bad stream index");
+    const int32_t row_off[2] = {0, n_phrases};
+    bool any = false;
+    if (pk_status ps = e->boost_upload("pk_stream_set_boost", s.boost, stream, 1, 0, phrase_ids, phrase_off, row_off, &boost, &any)) return ps;
+    s.n_boosted += (any ? 1 : 0) - (s.boosted[stream] ? 1 : 0);
+    s.boosted[stream] = any ? 1 : 0;
+    launch_boost_state_reset(s.boost.trie(), e->cfg.vocab, stream, 1, s.boost_bits, s.trie_active, s.trie_nact, e->stream);
+    const cudaError_t ce = cudaGetLastError();
+    if (ce != cudaSuccess) return e->fail(PK_ERR_CUDA, std::string("pk_stream_set_boost: ") + cudaGetErrorString(ce));
+    return PK_OK;
 }
 
 int32_t pk_stream_count(const pk_engine *e) { return (e && e->ss && !e->diar) ? e->ss->S : 0; }

@@ -55,6 +55,7 @@
 // shared memory.
 #include <cstdlib>
 #include <cstring>
+#include <map>
 
 #include "kernels.h"
 
@@ -352,7 +353,55 @@ __host__ __device__ inline TdtGeom tdt_geom(int P, int J, int NO, int n_clusters
     return q;
 }
 
-template <int CL>
+// bits = the tokens that continue one of the row's n active trie states (ContextTrie::get_boosted_tokens, phrase_boost.cpp:40-51)
+__device__ __forceinline__ void boost_mark_bits(const TrieRow &tr, const int32_t *act, int n, int V, uint32_t *bits) {
+    const int BW = (V + 31) >> 5;
+    for (int w = 0; w < BW; ++w) bits[w] = 0u;
+    for (int q = 0; q < n; ++q)
+        for (int e = tr.first[act[q]]; e < tr.first[act[q] + 1]; ++e) {
+            const int tk = tr.tok[e];
+            if (tk >= 0 && tk < V) bits[tk >> 5] |= 1u << (tk & 31);
+        }
+}
+// ContextTrie's initial state for row b: only the root is active; its children are the boosted tokens of the first step
+__device__ __forceinline__ void boost_row_reset(const DeviceTrie &trie, int V, int b, uint32_t *bits, int32_t *active, int32_t *nact) {
+    active[(size_t)b * BOOST_MAX_ACTIVE] = 0;
+    nact[b] = 1;
+    boost_mark_bits(trie_row(trie, b), active + (size_t)b * BOOST_MAX_ACTIVE, 1, V, bits + (size_t)b * ((V + 31) >> 5));
+}
+
+// Row b emitted `token` with the boosted score `key`: ContextTrie::advance (phrase_boost.cpp:53-66) on the row's active states
+// and the bitmap of the next step's boosted tokens; returns the token's raw logit.  A row with an empty trie has no state.
+// (Not inlined: it runs once per emitted token in one CTA and must not cost the decode loop registers.)
+__device__ __noinline__ float boost_advance(const DeviceTrie &trie, int b, int token, float key, int V, uint32_t *boost_bits,
+                                            int32_t *trie_active, int32_t *trie_nact) {
+    const TrieRow tr = trie_row(trie, b);
+    if (tr.empty()) return key;
+    uint32_t *bits = boost_bits + (size_t)b * ((V + 31) >> 5);
+    const float raw = ((bits[token >> 5] >> (token & 31)) & 1u) ? key - tr.boost : key;
+    int32_t *act = trie_active + (size_t)b * BOOST_MAX_ACTIVE;
+    const int na = trie_nact[b];
+    int32_t nxt[BOOST_MAX_ACTIVE];
+    int nn = 1;
+    nxt[0] = 0;
+    for (int a = 0; a < na; ++a) {
+        const int node = act[a];
+        for (int e = tr.first[node]; e < tr.first[node + 1]; ++e)
+            if (tr.tok[e] == token) {
+                const int ch = tr.child[e];
+                bool dup = false;
+                for (int q = 0; q < nn; ++q) dup |= nxt[q] == ch;
+                if (!dup && nn < BOOST_MAX_ACTIVE) nxt[nn++] = ch;
+            }
+    }
+    for (int q = 0; q < nn; ++q) act[q] = nxt[q];
+    trie_nact[b] = nn;
+    boost_mark_bits(tr, act, nn, V, bits);
+    return raw;
+}
+
+// BOOST = p.boost_on as a compile-time constant: the unboosted decode carries none of the boosting code or its registers.
+template <int CL, bool BOOST>
 __global__ void __launch_bounds__(NTHR, 1) tdt_decode_kernel(TdtParams p) {
     extern __shared__ __align__(16) float sm[];
     const int G = gridDim.x, g = blockIdx.x, tid = threadIdx.x;
@@ -501,7 +550,9 @@ __global__ void __launch_bounds__(NTHR, 1) tdt_decode_kernel(TdtParams p) {
                 if (m[i] > -INFINITY) s += sv[i] * expf(m[i] - gmax);
             s = warp_sum(s);
             // exp(log-prob of the emitted token); without boosting the token IS the maximum: exp(0) / s
-            if (lane == 0) p.t_conf[(size_t)b * p.cap + slot] = p.boost_on ? expf(s_vraw[b] - gmax) / s : 1.0f / s;
+            // (a row with an empty trie takes the unboosted form: the same bits as a decode with boosting off)
+            if (lane == 0)
+                p.t_conf[(size_t)b * p.cap + slot] = (BOOST && !trie_row(p.trie, b).empty()) ? expf(s_vraw[b] - gmax) / s : 1.0f / s;
         }
     };
     auto nox = [&](int) { return static_cast<const bf16 *>(nullptr); };
@@ -653,8 +704,10 @@ __global__ void __launch_bounds__(NTHR, 1) tdt_decode_kernel(TdtParams p) {
                             } else {
                                 lsum += expf(v - lmax);
                             }
-                            if (p.boost_on && bc + tid < Bpad) {
-                                const float vb = v + (((p.boost_bits[(size_t)(bc + tid) * BW + (n >> 5)] >> (n & 31)) & 1u) ? p.boost : 0.0f);
+                            if (BOOST && bc + tid < Bpad) {
+                                // (bits are set only by a row's own reset / advance, so a set bit means b < n_utt of some launch and its slot exists;
+                                // padding rows stay zero from the allocation.  The score is fetched only where one is added)
+                                const float vb = ((p.boost_bits[(size_t)(bc + tid) * BW + (n >> 5)] >> (n & 31)) & 1u) ? v + trie_row(p.trie, bc + tid).boost : v;
                                 if (vb > kmax) {         // rows ascend within a CTA: strict '>' keeps the first maximum
                                     kmax = vb;
                                     kidx = n;
@@ -674,7 +727,7 @@ __global__ void __launch_bounds__(NTHR, 1) tdt_decode_kernel(TdtParams p) {
                 p.pl_max[kb * PB + (size_t)g * Bpad + b] = lmax;
                 p.pl_sum[kb * PB + (size_t)g * Bpad + b] = lsum;
                 if (b < p.n_utt && s_active[b]) {
-                    if (p.boost_on) {
+                    if (BOOST) {
                         if (kmax > -INFINITY) atomicMax(&p.key_lab[kb * KB + b], pack_key(kmax, kidx));
                     } else if (lmax > -INFINITY) {
                         atomicMax(&p.key_lab[kb * KB + b], pack_key(lmax, lidx));
@@ -714,36 +767,10 @@ __global__ void __launch_bounds__(NTHR, 1) tdt_decode_kernel(TdtParams p) {
                     row[0] = n + 1;
                 }
                 if (n < p.cap) s_pend[b] = n;
-                if (p.boost_on && (b % G) == g) {
+                if (BOOST && (b % G) == g) {
                     // raw logit of the emitted token (its key carries the boosted value), then ContextTrie::advance
                     // (phrase_boost.cpp:53-66) and the bitmap of the next step's boosted tokens (:40-51)
-                    const int BW = (V + 31) >> 5;
-                    uint32_t *bits = p.boost_bits + (size_t)b * BW;
-                    s_vraw[b] = ((bits[lidx >> 5] >> (lidx & 31)) & 1u) ? lmax - p.boost : lmax;
-                    int32_t *act = p.trie_active + (size_t)b * 64;
-                    const int na = p.trie_nact[b];
-                    int32_t nxt[64];
-                    int nn = 1;
-                    nxt[0] = 0;
-                    for (int a = 0; a < na; ++a) {
-                        const int node = act[a];
-                        for (int e2 = p.trie.first[node]; e2 < p.trie.first[node + 1]; ++e2)
-                            if (p.trie.tok[e2] == lidx) {
-                                const int ch = p.trie.child[e2];
-                                bool dup = false;
-                                for (int q = 0; q < nn; ++q) dup |= nxt[q] == ch;
-                                if (!dup && nn < 64) nxt[nn++] = ch;
-                            }
-                    }
-                    for (int w = 0; w < BW; ++w) bits[w] = 0u;
-                    for (int q = 0; q < nn; ++q) {
-                        act[q] = nxt[q];
-                        for (int e2 = p.trie.first[nxt[q]]; e2 < p.trie.first[nxt[q] + 1]; ++e2) {
-                            const int tk = p.trie.tok[e2];
-                            if (tk >= 0 && tk < V) bits[tk >> 5] |= 1u << (tk & 31);
-                        }
-                    }
-                    p.trie_nact[b] = nn;
+                    s_vraw[b] = boost_advance(p.trie, b, lidx, lmax, V, p.boost_bits, p.trie_active, p.trie_nact);
                 }
                 s_ntok[b] = n + 1;
                 s_token[b] = lidx;
@@ -805,18 +832,13 @@ __global__ void tdt_init_kernel(TdtParams p) {
     if (b < p.n_utt) {
         p.tok[(size_t)b * (1 + p.cap)] = 0;
         p.overflow[b] = 0;
-        if (p.boost_on) {     // ContextTrie: only the root is active; its children are the boosted tokens of the first step
-            const int BW = (p.V + 31) >> 5;
-            uint32_t *bits = p.boost_bits + (size_t)b * BW;
-            for (int w = 0; w < BW; ++w) bits[w] = 0u;
-            for (int e = p.trie.first[0]; e < p.trie.first[1]; ++e) {
-                const int tk = p.trie.tok[e];
-                if (tk >= 0 && tk < p.V) bits[tk >> 5] |= 1u << (tk & 31);
-            }
-            p.trie_active[(size_t)b * 64] = 0;
-            p.trie_nact[b] = 1;
-        }
+        if (p.boost_on && !p.carry) boost_row_reset(p.trie, p.V, b, p.boost_bits, p.trie_active, p.trie_nact);
     }
+}
+
+__global__ void boost_state_reset_kernel(DeviceTrie trie, int V, int row0, int n, uint32_t *bits, int32_t *active, int32_t *nact) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) boost_row_reset(trie, V, row0 + i, bits, active, nact);
 }
 
 // fp32 rows [rows][K] -> pre-split rows [rows][2 K] = [hi: K][lo: K] bf16
@@ -872,6 +894,7 @@ size_t tdt_smem_bytes(const TdtParams &p, int n_clusters, int CL, bool *out_in_s
 template <int CL>
 cudaError_t launch_cl(TdtParams p, int num_sms, cudaStream_t st, bool *fits, TdtLaunchCtl *ctl) {
     *fits = false;
+    const auto kernel = p.boost_on ? tdt_decode_kernel<CL, true> : tdt_decode_kernel<CL, false>;
     if (p.P % (16 * CL) || p.J % (16 * CL)) return cudaSuccess;
     // upper bound on clusters; the occupancy query below says how many can be co-resident
     int nc = num_sms / CL;
@@ -894,12 +917,12 @@ cudaError_t launch_cl(TdtParams p, int num_sms, cudaStream_t st, bool *fits, Tdt
         int lstm_floats, wstage_rows;
         const size_t smem = tdt_smem_bytes(p, nc, CL, &out_in_smem, &wih_in_smem, &lstm_floats, &wstage_rows);
         if (smem > 227 * 1024) return cudaSuccess;
-        err = cudaFuncSetAttribute(tdt_decode_kernel<CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (err != cudaSuccess) { cudaGetLastError(); return cudaSuccess; }
         cfg.gridDim = dim3(nc * CL);
         cfg.dynamicSmemBytes = smem;
         int max_clusters = 0;
-        err = cudaOccupancyMaxActiveClusters(&max_clusters, tdt_decode_kernel<CL>, &cfg);
+        err = cudaOccupancyMaxActiveClusters(&max_clusters, kernel, &cfg);
         if (err != cudaSuccess) { cudaGetLastError(); return cudaSuccess; }
         if (max_clusters >= nc) {
             p.out_in_smem = out_in_smem ? 1 : 0;
@@ -915,7 +938,7 @@ cudaError_t launch_cl(TdtParams p, int num_sms, cudaStream_t st, bool *fits, Tdt
                 ctl->staged_ih = !p.wih_in_smem && p.L > 1 && p.wstage_rows >= nU0 * 4 && nU0 <= RG / 4 && ge.KSP == ge.KSJ;
             }
             tdt_init_kernel<<<((3 * p.Bpad > GBAR * GBAR_STRIDE ? 3 * p.Bpad : GBAR * GBAR_STRIDE) + 127) / 128, 128, 0, st>>>(p);
-            return cudaLaunchKernelEx(&cfg, tdt_decode_kernel<CL>, p);
+            return cudaLaunchKernelEx(&cfg, kernel, p);
         }
         if (max_clusters < 1) return cudaSuccess;
         nc = max_clusters;                           // retry with what fits (geometry and smem change with nc)
@@ -931,6 +954,41 @@ void tdt_pass_profile(long long *out8, bool reset) {
         long long z[8] = {0, 0, 0, 0, 0, 0, 0, 0};
         cudaMemcpyToSymbol(g_pass_clk, z, sizeof(z));
     }
+}
+
+bool boost_trie_csr(const int32_t *phrase_ids, const int32_t *phrase_off, int32_t p0, int32_t p1, std::vector<int32_t> &first,
+                    std::vector<int32_t> &tok, std::vector<int32_t> &child) {
+    std::vector<std::map<int32_t, int32_t>> ch(1);
+    for (int32_t p = p0; p < p1; ++p) {
+        int32_t node = 0;
+        if (phrase_off[p + 1] < phrase_off[p]) return false;
+        for (int32_t i = phrase_off[p]; i < phrase_off[p + 1]; ++i) {
+            auto it = ch[node].find(phrase_ids[i]);
+            if (it == ch[node].end()) {
+                const int32_t nx = (int32_t)ch.size();
+                ch[node][phrase_ids[i]] = nx;
+                ch.emplace_back();
+                node = nx;
+            } else {
+                node = it->second;
+            }
+        }
+    }
+    first.assign(ch.size() + 1, 0);
+    tok.clear();
+    child.clear();
+    for (size_t i = 0; i < ch.size(); ++i) {
+        for (auto &kv : ch[i]) {
+            tok.push_back(kv.first);
+            child.push_back(kv.second);
+        }
+        first[i + 1] = (int32_t)tok.size();
+    }
+    return true;
+}
+
+void launch_boost_state_reset(const DeviceTrie &trie, int V, int row0, int n, uint32_t *bits, int32_t *active, int32_t *nact, cudaStream_t st) {
+    if (n > 0) boost_state_reset_kernel<<<(n + 63) / 64, 64, 0, st>>>(trie, V, row0, n, bits, active, nact);
 }
 
 void launch_tdt_split_rows(const float *src, int rows, int K, bf16 *dst, cudaStream_t st) {

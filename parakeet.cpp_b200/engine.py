@@ -67,6 +67,21 @@ class TdtHookOut(C.Structure):
         [(n, C.c_int32) for n in ("steps", "grid", "cl", "upc", "opc", "out_in_smem", "wih_in_smem", "staged_ih", "wstage_rows")]
 
 
+class TdtBoostHookIn(C.Structure):
+    """pk_tdt_boost_hook_in (include/parakeet_b200.h)."""
+    _fields_ = [("dec", TdtHookIn), ("phrase_ids", C.POINTER(C.c_int32)), ("phrase_off", C.POINTER(C.c_int32)),
+                ("row_off", C.POINTER(C.c_int32)), ("boost", C.POINTER(C.c_float)),
+                ("trie_active0", C.POINTER(C.c_int32)), ("trie_nact0", C.POINTER(C.c_int32))]
+
+
+class TdtBoostHookOut(C.Structure):
+    """pk_tdt_boost_hook_out (include/parakeet_b200.h)."""
+    _fields_ = [("dec", TdtHookOut), ("trie_active", C.POINTER(C.c_int32)), ("trie_nact", C.POINTER(C.c_int32)),
+                ("boost_bits", C.POINTER(C.c_uint32))]
+
+
+BOOST_ROW_NODES = 1024   # PK_BOOST_ROW_NODES: trie nodes (root included) one row's phrase list may make
+
 EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_config_nemotron_600m", "pk_engine_create", "pk_engine_destroy", "pk_last_error",
            "pk_mel_frames", "pk_encoder_frames", "pk_mel", "pk_encode", "pk_decode", "pk_ctc_logprobs",
            "pk_transcribe_batch", "pk_stage_pcm", "pk_prefetch_pcm", "pk_run_staged", "pk_fetch_tokens", "pk_sync",
@@ -83,7 +98,7 @@ EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_co
            "pk_config_sortformer_117m", "pk_sortformer_create", "pk_sortformer_forward", "pk_diarize_batch", "pk_run_diarize_staged",
            "pk_fetch_probs", "pk_diar_segments", "pk_kernel_mha", "pk_kernel_speaker_head",
            "pk_diar_stream_open", "pk_diar_stream_reset", "pk_diar_stream_step", "pk_diar_stream_step_feats", "pk_diar_stream_speakers",
-           "pk_diar_stream_count"]
+           "pk_diar_stream_count", "pk_set_boost_rows", "pk_stream_set_boost", "pk_kernel_tdt_decode_boosted"]
 
 _lib = None
 
@@ -170,6 +185,9 @@ def load_library():
     L.pk_stream_step.argtypes = [vp, f32p, i64p, C.POINTER(_PkTokens), f32p, i32p, f32p, i32p]
     L.pk_stream_count.argtypes = [vp]
     L.pk_set_boost.argtypes = [vp, i32p, i32p, C.c_int32, C.c_float]
+    L.pk_set_boost_rows.argtypes = [vp, i32p, i32p, i32p, f32p, C.c_int32]
+    L.pk_stream_set_boost.argtypes = [vp, C.c_int32, i32p, i32p, C.c_int32, C.c_float]
+    L.pk_kernel_tdt_decode_boosted.argtypes = [C.c_int, C.POINTER(TdtBoostHookIn), C.POINTER(TdtBoostHookOut), i64p]
     L.pk_safetensors_probe.argtypes = [C.c_char_p, C.c_char_p, f32p, C.c_int64, i64p]
     L.pk_stage_pcm_rate.argtypes = [vp, f32p, i64p, C.c_int32, C.c_int32]
     L.pk_resample_batch.argtypes = [vp, f32p, i64p, C.c_int32, C.c_int32, C.c_int32, f32p, i64p]
@@ -807,6 +825,19 @@ class Engine:
             ids = np.zeros(1, np.int32)
         self._check(self.L.pk_set_boost(self.h, _i32p(ids), _i32p(off), len(phrases), float(boost)), "pk_set_boost")
 
+    def set_boost_rows(self, lists: Sequence[Sequence[Sequence[int]]], boosts: Sequence[float]):
+        """lists[i] = the phrases (token-id sequences) of utterance i of the following batches, boosts[i] its score; an
+        empty list leaves that utterance unboosted; no lists at all clears.  Replaces, and is replaced by, set_boost."""
+        assert len(lists) == len(boosts)
+        ids, off, row = pack_phrase_lists(lists)
+        self._check(self.L.pk_set_boost_rows(self.h, _i32p(ids), _i32p(off), _i32p(row), _f32p(np.asarray(list(boosts) or [0], np.float32)),
+                                             len(lists)), "pk_set_boost_rows")
+
+    def stream_set_boost(self, stream: int, phrases: Sequence[Sequence[int]], boost: float = 5.0):
+        """The phrase list of one open stream from its next step on (an empty list: none); its trie state restarts."""
+        ids, off, _ = pack_phrase_lists([phrases])
+        self._check(self.L.pk_stream_set_boost(self.h, stream, _i32p(ids), _i32p(off), len(phrases), float(boost)), "pk_stream_set_boost")
+
     # -- non-16 kHz input: converted on the device (SURVEY.md section 8f row 4)
     def stage_rate(self, pcms: Sequence[np.ndarray], src_rate: int):
         buf, off = _pack(pcms)
@@ -897,6 +928,18 @@ class Engine:
         p, rows, ints = C.c_void_p(), C.c_int32(), C.c_int32()
         self._check(self.L.pk_token_buffer(self.h, C.byref(p), C.byref(rows), C.byref(ints)), "pk_token_buffer")
         return int(p.value), rows.value, ints.value
+
+
+def pack_phrase_lists(lists):
+    """Phrase lists (one per row, each a list of token-id sequences) -> (phrase_ids, phrase_off, row_off) int32 arrays in the
+    layout of pk_set_boost_rows."""
+    phrases = [ph for lst in lists for ph in lst]
+    ids = np.array([t for ph in phrases for t in ph] or [0], np.int32)
+    off = np.zeros(len(phrases) + 1, np.int32)
+    off[1:] = np.cumsum([len(ph) for ph in phrases])
+    row = np.zeros(len(lists) + 1, np.int32)
+    row[1:] = np.cumsum([len(lst) for lst in lists])
+    return ids, off, row
 
 
 class Tokenizer:
@@ -1015,13 +1058,35 @@ class Transcriber:
         toks = self.engine.transcribe_batch([samples], self._decoder(opts.decoder))[0]
         return self._result(toks, opts.timestamps)
 
-    def transcribe_batch(self, audios, decoder=Decoder.TDT, timestamps: bool = False) -> List[TranscribeResult]:
+    def transcribe_batch(self, audios, decoder=Decoder.TDT, timestamps: bool = False,
+                         options: Optional[Sequence[TranscribeOptions]] = None) -> List[TranscribeResult]:
+        """options: one TranscribeOptions per utterance (decoder and timestamps must agree across the batch); each
+        utterance is decoded with its own boost_phrases / boost_score, as transcribe() would on it alone."""
         pcms = [read_wav(a) if isinstance(a, str) else np.asarray(a, np.float32) for a in audios]
+        lists = None
+        if options is not None:
+            if len(options) != len(pcms):
+                raise ValueError("transcribe_batch: one TranscribeOptions per utterance")
+            if any(o.decoder != options[0].decoder or o.timestamps != options[0].timestamps for o in options):
+                raise ValueError("transcribe_batch: decoder and timestamps must agree across the batch")
+            if options:
+                decoder, timestamps = options[0].decoder, options[0].timestamps
+            if any(o.boost_phrases for o in options):
+                if self.config.is_rnnt:
+                    raise ValueError("phrase boosting covers CTC and TDT decodes; this is an RNN-T model")
+                lists = [[self.tokenizer.encode(ph) for ph in o.boost_phrases] for o in options]
+                lists = [[ph for ph in lst if ph] for lst in lists]           # (ContextTrie::build skips phrases without tokens)
         out = []
         B = self.config.max_batch
         for i in range(0, len(pcms), B):
-            for toks in self.engine.transcribe_batch(pcms[i:i + B], self._decoder(decoder)):
-                out.append(self._result(toks, timestamps))
+            if lists is not None:
+                self.engine.set_boost_rows(lists[i:i + B], [o.boost_score for o in options[i:i + B]])
+            try:
+                for toks in self.engine.transcribe_batch(pcms[i:i + B], self._decoder(decoder)):
+                    out.append(self._result(toks, timestamps))
+            finally:
+                if lists is not None:
+                    self.engine.set_boost_rows([], [])
         return out
 
 
