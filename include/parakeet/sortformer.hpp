@@ -203,6 +203,7 @@ class Sortformer {
     }
 
     friend class DiarizationStreamingBatch;
+    friend class DiarizedTranscriber;
     // Sortformer::probs_to_segments (sortformer.cpp:70-113), pk_diar_segments
     std::vector<DiarizationSegment> probs_to_segments(const std::vector<float> &probs) const {
         const int32_t S = config_.max_speakers, T = (int32_t)(probs.size() / (size_t)S);

@@ -475,6 +475,30 @@ pk_status pk_fetch_probs(pk_engine *e, float *probs_out, int32_t *t_out);
  * p > threshold; a segment is [start frame, last active frame] in seconds (frame * 0.08 s); segments sorted by start, equal
  * starts by speaker id.  Writes at most cap segments; returns their full number, or -1 on invalid arguments. */
 int32_t pk_diar_segments(const float *probs, int32_t T, int32_t S, float threshold, int32_t *spk, float *start, float *end, int32_t cap);
+/* Speaker-attributed transcription (DiarizedTranscriber, include/parakeet/diarize.hpp; diarize.cpp of the reference): one batch
+ * through an ASR engine and a Sortformer engine on the same device.  The PCM is copied to the device once, into asr's buffer
+ * (pk_stage_pcm's staging); diar's front end reads it from there, and asr does not overwrite or swap that buffer (next
+ * pk_stage_pcm, pk_prefetch_pcm) before diar has read it.  tokens_out as pk_transcribe_batch on asr, probs_out / t_out as
+ * pk_diarize_batch on diar.  PK_ERR_INVALID: engines on different devices, asr a Sortformer or RNN-T engine, diar not a
+ * Sortformer engine, dec not CTC or TDT.  An n_utt or utterance length over either engine's capacity: PK_ERR_CAPACITY, with
+ * nothing staged.  Errors are reported by pk_last_error(asr).  Phrase boosting set on asr applies as in pk_transcribe_batch. */
+pk_status pk_transcribe_diarize_batch(pk_engine *asr, pk_engine *diar, const float *pcm, const int64_t *offsets, int32_t n_utt,
+                                      pk_decoder dec, pk_tokens *tokens_out, float *probs_out, int32_t *t_out);
+/* Device-resident form (measurement): pk_stage_pcm(asr, ...) (or pk_prefetch_pcm + pk_stage_pcm), then
+ * pk_run_transcribe_diarize_staged, then pk_fetch_tokens(asr) and pk_fetch_probs(diar).  diar keeps no PCM of this batch:
+ * pk_run_diarize_staged on it needs a pk_stage_pcm of its own first. */
+pk_status pk_run_transcribe_diarize_staged(pk_engine *asr, pk_engine *diar, pk_decoder dec);
+/* diarize_transcription (diarize.cpp:10-48) on the host: word w gets the speaker with the largest summed overlap
+ * min(end) - max(start) (float32 seconds; only overlaps > 0 count) over the segment list in its order, or -1 when none
+ * overlaps; exact ties resolve as the reference's std::unordered_map does (DESIGN.md section 13). */
+pk_status pk_diarize_transcription(const float *word_start, const float *word_end, int32_t n_words, const int32_t *seg_spk,
+                                   const float *seg_start, const float *seg_end, int32_t n_segs, int32_t *word_spk);
+/* One utterance of DiarizedTranscriber::transcribe after the models: the segments of probs [T][S] in the reference's own
+ * order (per speaker, then std::sort by start: above 16 segments equal starts need not stay in speaker order, unlike
+ * pk_diar_segments) -- at most seg_cap of them written -- and word_spk[n_words] from pk_diarize_transcription on them.
+ * Word times in seconds (pk_group_words).  Returns the number of segments, or -1 on invalid arguments. */
+int32_t pk_diarize_words(const float *probs, int32_t T, int32_t S, float threshold, const float *word_start, const float *word_end,
+                         int32_t n_words, int32_t *word_spk, int32_t *seg_spk, float *seg_start, float *seg_end, int32_t seg_cap);
 /* Streaming diarization: Sortformer::diarize_chunk (sortformer.cpp:124-150) with one EncoderCache and AOSCCache per stream,
  * n_streams streams in lock step on a Sortformer engine (the pk_stream_* conventions).  Per stream and step: the chunk's own
  * centred log-mel without normalisation (preprocess_audio(chunk, {n_mels = mel_bins, normalize = false}); nothing carries

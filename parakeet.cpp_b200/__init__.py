@@ -14,4 +14,5 @@ from .engine import (Decoder, Engine, ModelConfig, TranscribeOptions, Transcribe
                      make_tdt_600m_config, make_tiny_config, make_eou_120m_config, make_tiny_stream_config,
                      make_rnnt_600m_config, make_tiny_rnnt_config, make_nemotron_600m_config,
                      make_tiny_nemotron_config, SortformerConfig, DiarizationSegment, diar_segments,
-                     make_sortformer_117m_config, make_tiny_sortformer_config, AOSCCache)
+                     make_sortformer_117m_config, make_tiny_sortformer_config, AOSCCache, DiarizedWord,
+                     DiarizedResult, DiarizedTranscriber, diarize_transcription, diarize_words)

@@ -18,6 +18,7 @@
 #include "engine.h"
 
 #include <algorithm>
+#include <unordered_map>
 
 namespace pk_detail {
 std::string &create_err() {
@@ -1100,7 +1101,8 @@ static pk_status create_engine(const pk_config &c, const pk_sortformer_config *s
         ev_ok = cudaEventCreateWithFlags(&e->ev_chunk[i], cudaEventDisableTiming) == cudaSuccess;
     ev_ok = ev_ok && cudaEventCreateWithFlags(&e->ev_prefetch, cudaEventDisableTiming) == cudaSuccess &&
             cudaEventCreateWithFlags(&e->ev_pcm_free[0], cudaEventDisableTiming) == cudaSuccess &&
-            cudaEventCreateWithFlags(&e->ev_pcm_free[1], cudaEventDisableTiming) == cudaSuccess;
+            cudaEventCreateWithFlags(&e->ev_pcm_free[1], cudaEventDisableTiming) == cudaSuccess &&
+            cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming) == cudaSuccess;
     if (!ev_ok) {
         g_create_err = "cudaEventCreate / cudaStreamCreate failed";
         return PK_ERR_CUDA;
@@ -1154,6 +1156,7 @@ void pk_engine_destroy(pk_engine *e) {
     if (e->ev_prefetch) cudaEventDestroy(e->ev_prefetch);
     for (int i = 0; i < 2; ++i)
         if (e->ev_pcm_free[i]) cudaEventDestroy(e->ev_pcm_free[i]);
+    if (e->ev_join) cudaEventDestroy(e->ev_join);
     if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
     if (e->stream) cudaStreamDestroy(e->stream);
     delete e;
@@ -1703,6 +1706,7 @@ static pk_status run_pipeline(pk_engine *e, pk_decoder dec) {   // everything af
 
 // The ~250 launches of one batch are replayed as ONE CUDA graph once a batch shape has been seen
 // twice (first sight runs eagerly, which also completes every lazy one-time initialisation).
+static pk_status run_asr_graph(pk_engine *e, pk_decoder dec);
 pk_status pk_run_staged(pk_engine *e, pk_decoder dec) {
     if (!e || e->n_utt <= 0) return PK_ERR_INVALID;
     cudaSetDevice(e->device);
@@ -1713,6 +1717,10 @@ pk_status pk_run_staged(pk_engine *e, pk_decoder dec) {
         e->front_done = false;      // a second pk_run_staged of the same staged batch re-runs the front end
         if (fs) return fs;
     }
+    return run_asr_graph(e, dec);
+}
+
+static pk_status run_asr_graph(pk_engine *e, pk_decoder dec) {
     std::string key(1, dec == PK_DECODER_CTC ? 'c' : (dec == PK_DECODER_RNNT ? 'r' : 't'));
     // (per-row lists live in buffers that never move: one graph serves every set of lists)
     const int32_t bg = e->brows_on ? -1 : (e->boost_on ? e->boost_gen : 0);
@@ -2296,6 +2304,7 @@ pk_status pk_sortformer_forward(pk_engine *e, const float *feats, const int32_t 
 }
 
 // After pk_stage_pcm: the whole model after the front end replays as one CUDA graph per batch shape.
+static pk_status run_diar_graph(pk_engine *e);
 pk_status pk_run_diarize_staged(pk_engine *e) {
     if (!e || e->n_utt <= 0) return PK_ERR_INVALID;
     cudaSetDevice(e->device);
@@ -2305,6 +2314,10 @@ pk_status pk_run_diarize_staged(pk_engine *e) {
         e->front_done = false;
         if (fs) return fs;
     }
+    return run_diar_graph(e);
+}
+
+static pk_status run_diar_graph(pk_engine *e) {
     std::string key(1, 'd');
     key.append(reinterpret_cast<const char *>(e->frame_off.data()), e->frame_off.size() * sizeof(int32_t));
     pk_status s = e->run_graphed(key, [e]() {
@@ -2346,6 +2359,138 @@ int32_t pk_diar_segments(const float *probs, int32_t T, int32_t S, float thresho
         end[i] = (float)segs[i].t1 * 0.08f;
     }
     return (int32_t)segs.size();
+}
+
+// ===================================================================== speaker-attributed transcription (diarize.cpp)
+
+// DiarizedTranscriber holds a TDT-CTC Transcriber and a Sortformer (diarize.hpp of the reference): the pair must be an ASR
+// engine with a TDT joint and a Sortformer engine on one device, decoded with CTC or TDT.  Errors land on `asr`.
+static pk_status check_pair(pk_engine *asr, pk_engine *diar, pk_decoder dec) {
+    if (!asr || !diar) return PK_ERR_INVALID;
+    if (asr == diar || asr->diar) return asr->fail(PK_ERR_INVALID, "pk_transcribe_diarize: asr must be an ASR engine (pk_engine_create)");
+    if (asr->cfg.n_durations == 0) return asr->fail(PK_ERR_INVALID, "pk_transcribe_diarize: asr is an RNN-T model; a TDT-CTC or TDT model is needed");
+    if (!diar->diar) return asr->fail(PK_ERR_INVALID, "pk_transcribe_diarize: diar must be a Sortformer engine (pk_sortformer_create)");
+    if (asr->device != diar->device) return asr->fail(PK_ERR_INVALID, "pk_transcribe_diarize: the two engines are on different devices");
+    if (dec != PK_DECODER_CTC && dec != PK_DECODER_TDT) return asr->fail(PK_ERR_INVALID, "pk_transcribe_diarize: the decoder must be CTC or TDT");
+    if (asr->gemm_err) return asr->gemm_err;
+    if (diar->gemm_err) return asr->fail(diar->gemm_err, diar->err);
+    return PK_OK;
+}
+
+// The batch staged on `asr` (pk_stage_pcm, pk_prefetch_pcm adoption, pk_stage_pcm_rate or pk_job_select) through both
+// models.  The PCM is on the device once, in asr's buffer; diar's front end reads it there (pcm_src).
+//   asr stream : [front end] [ASR graph] (wait: diar's front end has read the PCM) [ev_pcm_free]
+//   diar stream: (wait: the PCM has landed) [front end] (wait: the ASR graph is done) [diarization graph]
+// Every later writer of asr's PCM buffers (pk_stage_pcm's copies on either stream, pk_prefetch_pcm's wait on ev_pcm_free)
+// is ordered after asr's stream at the ev_pcm_free record, so it cannot overwrite or swap the buffer before diar read it.
+pk_status pk_run_transcribe_diarize_staged(pk_engine *asr, pk_engine *diar, pk_decoder dec) {
+    if (pk_status s = check_pair(asr, diar, dec)) return s;
+    if (asr->n_utt <= 0) return asr->fail(PK_ERR_INVALID, "pk_run_transcribe_diarize_staged: no batch staged on asr");
+    cudaSetDevice(asr->device);
+    pk_status s;
+    if ((s = check_decoder(asr, dec))) return s;
+    const int n = asr->n_utt;
+    if ((s = diar->set_batch_shapes(nullptr, asr->pcm_off.data(), n)) || (s = diar->upload_shapes()))
+        return asr->fail(s, diar->err);
+    pk_engine *e = asr;    // (PK_ECUDA reports on e)
+    // The samples have landed once the staging copies have: on the copy stream when pk_stage_pcm already ran asr's front
+    // end under them (pinned buffer or adopted prefetch), else on asr's stream ahead of its (not yet launched) front end.
+    PK_ECUDA(cudaEventRecord(asr->ev_join, asr->front_done ? asr->copy_stream : asr->stream));
+    PK_ECUDA(cudaStreamWaitEvent(diar->stream, asr->ev_join, 0));
+    diar->pcm_src = asr->pcm_src ? asr->pcm_src : asr->d_pcm;
+    diar->front_done = false;
+    s = run_front(diar);
+    diar->pcm_src = nullptr;    // diar holds no PCM of its own for this batch
+    diar->front_done = false;
+    if (s) return asr->fail(s, diar->err);
+    PK_ECUDA(cudaEventRecord(diar->ev_join, diar->stream));
+    s = run_front(asr);
+    asr->front_done = false;
+    if (s == PK_OK) s = run_asr_graph(asr, dec);
+    // (also on failure: the buffer is not free before diar's front end has read it)
+    PK_ECUDA(cudaStreamWaitEvent(asr->stream, diar->ev_join, 0));
+    PK_ECUDA(cudaEventRecord(asr->ev_pcm_free[asr->pcm_cur], asr->stream));
+    if (s) return s;
+    // Back to back: the diarization graph starts when the ASR graph has finished (DESIGN.md section 13: running the two
+    // graphs side by side measured no faster).
+    PK_ECUDA(cudaEventRecord(asr->ev_join, asr->stream));
+    PK_ECUDA(cudaStreamWaitEvent(diar->stream, asr->ev_join, 0));
+    s = run_diar_graph(diar);
+    if (s) return asr->fail(s, diar->err);
+    return PK_OK;
+}
+
+pk_status pk_transcribe_diarize_batch(pk_engine *asr, pk_engine *diar, const float *pcm, const int64_t *offsets, int32_t n_utt,
+                                      pk_decoder dec, pk_tokens *tokens_out, float *probs_out, int32_t *t_out) {
+    if (!pcm || !offsets || !probs_out) return asr ? asr->fail(PK_ERR_INVALID, "pk_transcribe_diarize_batch: null argument") : PK_ERR_INVALID;
+    pk_status s;
+    if ((s = check_pair(asr, diar, dec))) return s;
+    if ((s = check_decoder(asr, dec))) return s;
+    // diar's capacity before anything is staged (host-side shapes only)
+    if ((s = diar->set_batch_shapes(nullptr, offsets, n_utt))) return asr->fail(s, diar->err);
+    if ((s = pk_stage_pcm(asr, pcm, offsets, n_utt))) return s;
+    if ((s = pk_run_transcribe_diarize_staged(asr, diar, dec))) return s;
+    if ((s = pk_fetch_tokens(asr, tokens_out))) return s;
+    if ((s = pk_fetch_probs(diar, probs_out, t_out))) return asr->fail(s, diar->err);
+    return PK_OK;
+}
+
+// diarize_transcription (diarize.cpp:10-48): per word, the overlap min(end) - max(start) with every segment in list order,
+// summed per speaker when > 0 in a std::unordered_map<int, float>, and the first speaker of the map's iteration with a
+// strictly larger sum wins.  The map is kept on purpose: on an exact tie the winner is whichever the container iterates
+// first (DESIGN.md section 13), and only the same container reproduces that.
+pk_status pk_diarize_transcription(const float *word_start, const float *word_end, int32_t n_words, const int32_t *seg_spk,
+                                   const float *seg_start, const float *seg_end, int32_t n_segs, int32_t *word_spk) {
+    if (n_words < 0 || n_segs < 0 || (n_words > 0 && (!word_start || !word_end || !word_spk)) ||
+        (n_segs > 0 && (!seg_spk || !seg_start || !seg_end)))
+        return PK_ERR_INVALID;
+    for (int32_t w = 0; w < n_words; ++w) {
+        std::unordered_map<int, float> overlap_by_speaker;
+        for (int32_t k = 0; k < n_segs; ++k) {
+            const float overlap = std::min(word_end[w], seg_end[k]) - std::max(word_start[w], seg_start[k]);
+            if (overlap > 0.0f) overlap_by_speaker[seg_spk[k]] += overlap;
+        }
+        float best = 0.0f;
+        int32_t id = -1;
+        for (const auto &kv : overlap_by_speaker)
+            if (kv.second > best) {
+                best = kv.second;
+                id = kv.first;
+            }
+        word_spk[w] = id;
+    }
+    return PK_OK;
+}
+
+// Sortformer::probs_to_segments (sortformer.cpp:70-113) in the reference's own order -- built per speaker, then sorted by
+// start with std::sort, whose introsort reorders equal starts above 16 segments (pk_diar_segments keeps speaker order
+// instead) -- followed by pk_diarize_transcription on those segments.
+int32_t pk_diarize_words(const float *probs, int32_t T, int32_t S, float threshold, const float *word_start, const float *word_end,
+                         int32_t n_words, int32_t *word_spk, int32_t *seg_spk, float *seg_start, float *seg_end, int32_t seg_cap) {
+    if (!probs || T < 0 || S < 1 || seg_cap < 0 || (seg_cap > 0 && (!seg_spk || !seg_start || !seg_end))) return -1;
+    struct Seg { int32_t speaker_id; float start, end; };
+    std::vector<Seg> segs;
+    for (int s = 0; s < S; ++s) {
+        int t0 = -1;
+        for (int t = 0; t < T; ++t) {
+            const bool active = probs[(size_t)t * S + s] > threshold;
+            if (active && t0 < 0) t0 = t;
+            else if (!active && t0 >= 0) { segs.push_back({s, (float)t0 * 0.08f, (float)(t - 1) * 0.08f}); t0 = -1; }
+        }
+        if (t0 >= 0) segs.push_back({s, (float)t0 * 0.08f, (float)(T - 1) * 0.08f});
+    }
+    std::sort(segs.begin(), segs.end(), [](const Seg &a, const Seg &b) { return a.start < b.start; });
+    const int32_t ns = (int32_t)segs.size();
+    std::vector<int32_t> spk(ns);
+    std::vector<float> st(ns), en(ns);
+    for (int32_t i = 0; i < ns; ++i) {
+        spk[i] = segs[i].speaker_id;
+        st[i] = segs[i].start;
+        en[i] = segs[i].end;
+        if (i < seg_cap) { seg_spk[i] = spk[i]; seg_start[i] = st[i]; seg_end[i] = en[i]; }
+    }
+    if (pk_diarize_transcription(word_start, word_end, n_words, spk.data(), st.data(), en.data(), ns, word_spk) != PK_OK) return -1;
+    return ns;
 }
 
 }  // extern "C"

@@ -134,6 +134,7 @@ struct pk_engine {
     float *d_pcm_alt = nullptr;               // second PCM buffer (pk_prefetch_pcm); swapped with d_pcm on adoption
     cudaEvent_t ev_pcm_free[2] = {}, ev_prefetch = nullptr;   // [k]: last front end reading buffer k has run; prefetch copy done
     int pcm_cur = 0;                           // which physical buffer d_pcm currently is
+    cudaEvent_t ev_join = nullptr;             // pk_run_transcribe_diarize_staged: recorded here for the other engine of the pair to wait on
     struct { const float *pcm = nullptr; int32_t n = 0; std::vector<int64_t> off; bool valid = false; } pref;
     int64_t *d_pcm_off = nullptr;
     int32_t *d_frame_off = nullptr, *d_s2_off = nullptr, *d_row_off = nullptr, *d_t2_rows = nullptr;

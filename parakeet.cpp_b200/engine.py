@@ -16,7 +16,7 @@ import ctypes as C
 import enum
 import os
 import struct
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 from typing import List, Optional, Sequence
 
 import numpy as np
@@ -98,7 +98,8 @@ EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_co
            "pk_config_sortformer_117m", "pk_sortformer_create", "pk_sortformer_forward", "pk_diarize_batch", "pk_run_diarize_staged",
            "pk_fetch_probs", "pk_diar_segments", "pk_kernel_mha", "pk_kernel_speaker_head",
            "pk_diar_stream_open", "pk_diar_stream_reset", "pk_diar_stream_step", "pk_diar_stream_step_feats", "pk_diar_stream_speakers",
-           "pk_diar_stream_count", "pk_set_boost_rows", "pk_stream_set_boost", "pk_kernel_tdt_decode_boosted"]
+           "pk_diar_stream_count", "pk_set_boost_rows", "pk_stream_set_boost", "pk_kernel_tdt_decode_boosted",
+           "pk_transcribe_diarize_batch", "pk_run_transcribe_diarize_staged", "pk_diarize_transcription", "pk_diarize_words"]
 
 _lib = None
 
@@ -209,6 +210,11 @@ def load_library():
     L.pk_diar_stream_speakers.restype = C.c_int32
     L.pk_diar_stream_count.argtypes = [vp]
     L.pk_diar_stream_count.restype = C.c_int32
+    L.pk_transcribe_diarize_batch.argtypes = [vp, vp, f32p, i64p, C.c_int32, C.c_int, C.POINTER(_PkTokens), f32p, i32p]
+    L.pk_run_transcribe_diarize_staged.argtypes = [vp, vp, C.c_int]
+    L.pk_diarize_transcription.argtypes = [f32p, f32p, C.c_int32, i32p, f32p, f32p, C.c_int32, i32p]
+    L.pk_diarize_words.argtypes = [f32p, C.c_int32, C.c_int32, C.c_float, f32p, f32p, C.c_int32, i32p, i32p, f32p, f32p, C.c_int32]
+    L.pk_diarize_words.restype = C.c_int32
     _lib = L
     return L
 
@@ -769,6 +775,22 @@ class Engine:
     def fetch_probs(self, out: np.ndarray, lens: np.ndarray):
         self._check(self.L.pk_fetch_probs(self.h, _f32p(out), _i32p(lens)), "pk_fetch_probs")
 
+    # -- speaker-attributed transcription: this ASR engine and a Sortformer engine over one staged batch
+    def transcribe_diarize_batch(self, diar_engine: "Engine", pcms: Sequence[np.ndarray], decoder: Decoder):
+        """pk_transcribe_diarize_batch -> (tokens per utterance, activities [T'][max_speakers] per utterance)."""
+        buf, off = _pack(pcms)
+        t, arrs = self._tokens(len(pcms))
+        M = sum(self.L.pk_encoder_frames(self.L.pk_mel_frames(len(p))) for p in pcms)
+        probs = np.zeros((max(M, 1), diar_engine.cfg.max_speakers), np.float32)
+        lens = np.zeros(max(len(pcms), 1), np.int32)
+        self._check(self.L.pk_transcribe_diarize_batch(self.h, diar_engine.h, _f32p(buf), _i64p(off), len(pcms), int(decoder),
+                                                        C.byref(t), _f32p(probs), _i32p(lens)), "pk_transcribe_diarize_batch")
+        return self._unpack(arrs, len(pcms)), self._probs(lens[:len(pcms)], probs)
+
+    def run_transcribe_diarize_staged(self, diar_engine: "Engine", decoder: Decoder):
+        """After stage() on this engine: both models on the staged batch (then fetch / fetch_probs on each engine)."""
+        self._check(self.L.pk_run_transcribe_diarize_staged(self.h, diar_engine.h, int(decoder)), "pk_run_transcribe_diarize_staged")
+
     # -- streaming diarization (a Sortformer engine): Sortformer::diarize_chunk for n_streams streams in lock step
     def diar_stream_open(self, n_streams: int, max_chunk_samples: int = 16000, att_context_left: int = 70):
         self._check(self.L.pk_diar_stream_open(self.h, n_streams, max_chunk_samples, att_context_left), "pk_diar_stream_open")
@@ -1087,6 +1109,98 @@ class Transcriber:
             finally:
                 if lists is not None:
                     self.engine.set_boost_rows([], [])
+        return out
+
+
+@dataclass
+class DiarizedWord:                   # diarize.hpp:19-25
+    word: str
+    start: float                      # seconds
+    end: float
+    speaker_id: int = -1              # -1: no overlapping segment
+    confidence: float = 1.0
+
+
+@dataclass
+class DiarizedResult:                 # diarize.hpp:27-32
+    text: str = ""
+    words: List[DiarizedWord] = field(default_factory=list)
+    segments: List[DiarizationSegment] = field(default_factory=list)
+    word_timestamps: List[WordTimestamp] = field(default_factory=list)
+
+
+def diarize_transcription(words: Sequence[WordTimestamp], segments: Sequence[DiarizationSegment]) -> List[DiarizedWord]:
+    """diarize_transcription (reference diarize.cpp:10-48), pk_diarize_transcription: each word gets the speaker with the
+    largest summed overlap over the segments in list order (ties as the reference's std::unordered_map), or -1."""
+    L = load_library()
+    ws = np.array([w.start for w in words] or [0], np.float32)
+    we = np.array([w.end for w in words] or [0], np.float32)
+    spk = np.array([s.speaker_id for s in segments] or [0], np.int32)
+    ss = np.array([s.start for s in segments] or [0], np.float32)
+    se = np.array([s.end for s in segments] or [0], np.float32)
+    out = np.zeros(max(len(words), 1), np.int32)
+    if L.pk_diarize_transcription(_f32p(ws), _f32p(we), len(words), _i32p(spk), _f32p(ss), _f32p(se), len(segments), _i32p(out)) != 0:
+        raise RuntimeError("pk_diarize_transcription: invalid arguments")
+    return [DiarizedWord(w.word, w.start, w.end, int(out[i]), w.confidence) for i, w in enumerate(words)]
+
+
+def diarize_words(probs: np.ndarray, words: Sequence[WordTimestamp], threshold: float = 0.5):
+    """pk_diarize_words on one utterance: -> (segments in the reference's order, [DiarizedWord])."""
+    L = load_library()
+    p = np.ascontiguousarray(probs, np.float32)
+    T, S = p.shape
+    ws = np.array([w.start for w in words] or [0], np.float32)
+    we = np.array([w.end for w in words] or [0], np.float32)
+    spk = np.zeros(max(len(words), 1), np.int32)
+    cap = T * S // 2 + S
+    ss, st, en = np.zeros(cap, np.int32), np.zeros(cap, np.float32), np.zeros(cap, np.float32)
+    n = L.pk_diarize_words(_f32p(p), T, S, float(threshold), _f32p(ws), _f32p(we), len(words), _i32p(spk), _i32p(ss), _f32p(st),
+                           _f32p(en), cap)
+    if n < 0:
+        raise RuntimeError("pk_diarize_words: invalid arguments")
+    segs = [DiarizationSegment(int(ss[i]), float(st[i]), float(en[i])) for i in range(n)]
+    return segs, [DiarizedWord(w.word, w.start, w.end, int(spk[i]), w.confidence) for i, w in enumerate(words)]
+
+
+class DiarizedTranscriber:
+    """Python mirror of parakeet::DiarizedTranscriber (include/parakeet/diarize.hpp): a TDT-CTC ASR engine and a Sortformer
+    engine with one capacity (max_batch utterances of max_samples), run over one staged batch (pk_transcribe_diarize_batch)."""
+
+    def __init__(self, asr_weights: str, sortformer_weights: str, vocab_path: str, config: Optional[ModelConfig] = None,
+                 sf_config: Optional[SortformerConfig] = None, device: int = 0, max_batch: int = 16, max_samples: int = 30 * 16000,
+                 math: int = 0):
+        cap = dict(max_batch=max_batch, max_samples=max_samples, math=math)
+        self.config = replace(config or make_110m_config(), **cap)
+        if self.config.is_rnnt:
+            raise ValueError("DiarizedTranscriber: the ASR model must be a TDT-CTC or TDT model")
+        sf = sf_config or make_sortformer_117m_config()
+        self.sf_config = replace(sf, encoder=replace(sf.encoder, **cap))
+        self.asr = Engine(self.config, asr_weights, device)
+        self.diar = Engine(self.sf_config, sortformer_weights, device)
+        self.tokenizer = Tokenizer(vocab_path)
+
+    def to_gpu(self):
+        """A no-op: both models only ever live on the CUDA device."""
+        return self
+
+    def close(self):
+        self.asr.close()
+        self.diar.close()
+
+    def transcribe(self, audio, decoder=Decoder.TDT) -> DiarizedResult:
+        return self.transcribe_batch([audio], decoder)[0]
+
+    def transcribe_batch(self, audios, decoder=Decoder.TDT) -> List[DiarizedResult]:
+        pcms = [read_wav(a) if isinstance(a, str) else np.asarray(a, np.float32) for a in audios]
+        dec = decoder if self.config.has_ctc else Decoder.TDT
+        out = []
+        B = self.config.max_batch
+        for i in range(0, len(pcms), B):
+            toks, probs = self.asr.transcribe_diarize_batch(self.diar, pcms[i:i + B], dec)
+            for tk, p in zip(toks, probs):
+                wts = self.tokenizer.group_words(tk)
+                segs, words = diarize_words(p, wts, self.sf_config.activity_threshold)
+                out.append(DiarizedResult(self.tokenizer.decode([t.token_id for t in tk]), words, segs, wts))
         return out
 
 
