@@ -87,12 +87,15 @@ struct TranscribeResult {
     std::vector<TimestampedToken> timestamped_tokens;
     std::vector<WordTimestamp> word_timestamps;
 };
-enum class Decoder { CTC, TDT };
+// CTC_BEAM (not in the reference): CTC prefix beam search of beam_width hypotheses, fused with the language model of
+// Transcriber::set_language_model when one is set (pk_set_ctc_beam).  It does not combine with boost_phrases.
+enum class Decoder { CTC, TDT, CTC_BEAM };
 struct TranscribeOptions {
     Decoder decoder = Decoder::TDT;
     bool timestamps = false;
     std::vector<std::string> boost_phrases;
     float boost_score = 5.0f;
+    int beam_width = 8;
 };
 
 // ─── Tokenizer (vocab.hpp) over the C-ABI host helpers ───────────────────────
@@ -108,6 +111,7 @@ class Tokenizer {
         if (pk_vocab_load(vocab_path.c_str(), &v_) != PK_OK) throw std::runtime_error("Cannot open vocab file: " + vocab_path);
     }
     bool loaded() const { return v_ && pk_vocab_size(v_) > 0; }
+    const pk_vocab *handle() const { return v_; }   // for pk_set_ctc_beam
     size_t vocab_size() const { return loaded() ? (size_t)pk_vocab_size(v_) + 1 : 0; }   // +1 blank, like the reference
     std::string decode(const std::vector<int> &ids) const {
         std::vector<int32_t> a(ids.begin(), ids.end());
@@ -259,6 +263,7 @@ inline void check_batch_options(const std::vector<TranscribeOptions> &opts, size
     for (const auto &o : opts) {
         if (o.decoder != opts[0].decoder) throw std::invalid_argument("transcribe_batch: every utterance of a batch must name the same decoder");
         if (o.timestamps != opts[0].timestamps) throw std::invalid_argument("transcribe_batch: timestamps must be the same for every utterance of a batch");
+        if (o.beam_width != opts[0].beam_width) throw std::invalid_argument("transcribe_batch: every utterance of a batch must name the same beam width");
         if (rnnt_model && !o.boost_phrases.empty())
             throw std::runtime_error("RNNTTranscriber: phrase boosting covers CTC and TDT decodes only (phrase_boost.hpp)");
     }
@@ -366,12 +371,14 @@ class TranscriberBase {
                 guard.on = true;
             }
         }
+        setup_beam(opts.decoder, opts.beam_width, !opts.boost_phrases.empty());
         auto toks = eng_->run({samples}, {n}, self().pick(opts.decoder), sample_rate)[0];
         return finish(toks, opts.timestamps);
     }
     // Not in the reference (batch-1 only): one call for many utterances.
     std::vector<TranscribeResult> transcribe_batch(const std::vector<std::vector<float>> &utts, Decoder decoder = Decoder::TDT, bool timestamps = false) {
         std::vector<TranscribeResult> out;
+        setup_beam(decoder, TranscribeOptions().beam_width, false);
         const size_t B = (size_t)eng_->cfg().max_batch;
         for (size_t i = 0; i < utts.size(); i += B) {
             std::vector<const float *> p;
@@ -387,6 +394,9 @@ class TranscriberBase {
         check_batch_options(opts, utts.size(), eng_->cfg().n_durations == 0);
         std::vector<TranscribeResult> out;
         if (utts.empty()) return out;
+        bool boosted = false;
+        for (const auto &o : opts) boosted |= !o.boost_phrases.empty();
+        setup_beam(opts[0].decoder, opts[0].beam_width, boosted);
         struct RowsGuard {
             pk_engine *e; bool on;
             ~RowsGuard() { if (on) pk_set_boost_rows(e, nullptr, nullptr, nullptr, nullptr, 0); }
@@ -418,6 +428,23 @@ class TranscriberBase {
     pk_engine *engine() { return eng_->raw(); }
 
   protected:
+    // Decoder::CTC_BEAM on a model that decodes it: the width and the language model go to the engine before the run, only
+    // when they differ from what the engine last got (set_language_model / clear_language_model mark them changed).
+    void setup_beam(Decoder d, int width, bool boosted) {
+        if (d != Decoder::CTC_BEAM || self().pick(d) != PK_DECODER_CTC_BEAM) return;
+        if (boosted) throw std::invalid_argument("Decoder::CTC_BEAM does not take boost_phrases");
+        if (width < 1 || width > PK_CTC_BEAM_MAX) throw std::invalid_argument("beam_width must be in 1.." + std::to_string(PK_CTC_BEAM_MAX));
+        if (!beam_dirty_ && width == beam_width_) return;
+        if (pk_set_ctc_beam(eng_->raw(), width, lm_.get(), lm_ ? tokenizer_.handle() : nullptr, lm_alpha_, lm_beta_) != PK_OK)
+            throw std::runtime_error(std::string("parakeet_b200: ") + pk_last_error(eng_->raw()));
+        beam_width_ = width;
+        beam_dirty_ = false;
+    }
+    struct LmFree { void operator()(pk_lm *p) const { pk_lm_free(p); } };
+    std::unique_ptr<pk_lm, LmFree> lm_;
+    float lm_alpha_ = 0.5f, lm_beta_ = 1.0f;
+    int beam_width_ = 0;
+    bool beam_dirty_ = true;
     TranscribeResult finish(const std::vector<TimestampedToken> &toks, bool timestamps) {
         TranscribeResult r;
         for (auto &t : toks) r.token_ids.push_back(t.token_id);
@@ -460,7 +487,20 @@ class Transcriber : public detail::TranscriberBase<Transcriber> {
         TranscribeOptions o; o.decoder = decoder; o.timestamps = timestamps;
         return TranscriberBase::transcribe(samples, n, o);
     }
-    pk_decoder pick(Decoder d) const { return d == Decoder::CTC ? PK_DECODER_CTC : PK_DECODER_TDT; }
+    pk_decoder pick(Decoder d) const { return d == Decoder::CTC ? PK_DECODER_CTC : (d == Decoder::CTC_BEAM ? PK_DECODER_CTC_BEAM : PK_DECODER_TDT); }
+    // Word n-gram LM (ARPA) for Decoder::CTC_BEAM: score = ln P(prefix) + alpha ln(10) sum log10 p(word | history) + beta words.
+    void set_language_model(const std::string &arpa_path, float alpha = 0.5f, float beta = 1.0f) {
+        pk_lm *p = nullptr;
+        if (pk_lm_load(arpa_path.c_str(), &p) != PK_OK) throw std::runtime_error(std::string("parakeet_b200: ") + pk_last_error(nullptr));
+        lm_.reset(p);
+        lm_alpha_ = alpha;
+        lm_beta_ = beta;
+        beam_dirty_ = true;
+    }
+    void clear_language_model() {
+        lm_.reset();
+        beam_dirty_ = true;
+    }
 };
 
 /// parakeet::TDTTranscriber (reference transcribe.hpp:200-299): TDT-only models (600M multilingual).

@@ -38,8 +38,9 @@ typedef enum {
 } pk_status;
 
 /* PK_DECODER_TDT runs only on a TDT model, PK_DECODER_RNNT only on an RNN-T model (n_durations = 0);
- * PK_DECODER_CTC needs a CTC head (has_ctc).  A mismatch is PK_ERR_INVALID. */
-typedef enum { PK_DECODER_CTC = 0, PK_DECODER_TDT = 1, PK_DECODER_RNNT = 2 } pk_decoder;
+ * PK_DECODER_CTC needs a CTC head (has_ctc).  A mismatch is PK_ERR_INVALID.  PK_DECODER_CTC_BEAM: CTC prefix beam
+ * search with optional word n-gram fusion (pk_set_ctc_beam below; DESIGN.md section 14). */
+typedef enum { PK_DECODER_CTC = 0, PK_DECODER_TDT = 1, PK_DECODER_RNNT = 2, PK_DECODER_CTC_BEAM = 3 } pk_decoder;
 
 /* GEMM arithmetic.  PK_MATH_BF16X3 (default): wgmma MMAs on bf16
  * hi/lo operand splits, 3 MMAs per product (hi*hi + hi*lo + lo*hi), fp32
@@ -440,6 +441,47 @@ pk_status pk_set_boost_rows(pk_engine *e, const int32_t *phrase_ids, const int32
  * the root, keeping the list (DESIGN.md section 8). */
 pk_status pk_stream_set_boost(pk_engine *e, int32_t stream, const int32_t *phrase_ids, const int32_t *phrase_off,
                               int32_t n_phrases, float boost);
+
+/* ---- CTC prefix beam search with word n-gram (ARPA) shallow fusion (DESIGN.md section 14 defines the decode).
+ * Per frame every beam is extended by the `width` best non-blank tokens of the frame; candidates with the same token
+ * sequence merge; each is ranked by ln P(prefix) + lm, lm = alpha ln(10) sum log10 p(word | history) + beta (words scored),
+ * over the completed words (a piece starting with U+2581 starts a word; words are the UTF-8 of their pieces without that
+ * mark, compared as bytes; a word the LM lacks scores as <unk>).  At the end the unfinished word and </s> are scored and the
+ * best beam is backtracked into the greedy layout of pk_tokens (start = frame the token was appended, end = next start - 1,
+ * conf = exp(log-prob at start)).
+ *
+ * The LM is a host object: pk_lm_load reads an ARPA file of order 1..6 (\data\ counts, \k-grams: sections of
+ * "log10prob w1 .. wk [log10backoff]", \end\).  PK_ERR_IO, with the line in pk_last_error(NULL), for a count that does not
+ * match its section, an n-gram whose context (or word) is not in the file, a field that does not parse, a missing \end\,
+ * or two words with the same 64-bit FNV-1a hash.  Without <unk> one is added (log10 p = -10, backoff 0).  Scoring is
+ * standard ARPA back-off from the longest present suffix of the history, starting from the <s> unigram when present.
+ *   pk_lm_count          : number of n-grams of `order` (1..pk_lm_order), <unk> included when it was added.
+ *   pk_lm_sentence_log10 : log10 p of the space-separated words followed by </s>, starting from <s> (NaN: bad argument).
+ *   pk_set_ctc_beam      : the beam width (1..PK_CTC_BEAM_MAX) for PK_DECODER_CTC_BEAM on this engine, and the LM (NULL:
+ *                          none; then vocab may be NULL and alpha / beta are unused) with the tokenizer whose pieces the
+ *                          model emits.  The LM's tables are copied to the device, so the pk_lm may be freed afterwards.
+ *                          They are copied only when the LM (a new pk_lm_load) or the vocabulary's pieces differ from the
+ *                          tables in place: that call synchronises the engine stream and frees the previous tables.  A call
+ *                          that repeats the LM and vocabulary (say, once per request) copies nothing and does not
+ *                          synchronise; width, alpha and beta may change on any call.  PK_DECODER_CTC_BEAM is PK_ERR_INVALID before this call, on a
+ *                          model without a CTC head, on a Sortformer engine, and while phrase boosting is set. */
+#define PK_CTC_BEAM_MAX 32
+typedef struct pk_lm pk_lm;
+pk_status pk_lm_load(const char *arpa_path, pk_lm **out);
+void pk_lm_free(pk_lm *lm);
+int32_t pk_lm_order(const pk_lm *lm);
+int64_t pk_lm_count(const pk_lm *lm, int32_t order);
+double pk_lm_sentence_log10(const pk_lm *lm, const char *space_separated_words);
+pk_status pk_set_ctc_beam(pk_engine *e, int32_t width, const pk_lm *lm_or_null, const pk_vocab *vocab, float alpha, float beta);
+/* Kernel test hook (conventions of the pk_kernel_* hooks): the two beam-search kernels as the engine launches them, on host
+ * log-probs [rows][V] (blank = V - 1), utterance b = rows [row_off[b], row_off[b+1]).  lm / vocab as pk_set_ctc_beam.
+ * Outputs, all guarded: tok [n_utt][1 + cap] (len, ids), t_start / t_end / t_conf [n_utt][cap], topk_id / topk_lp
+ * [rows][width] (absent entries: id -1), blank_lp [rows], bp [rows][width] (back-pointers: parent slot << 24 | (token + 1),
+ * written for the slots alive after each frame).  Any output but tok may be NULL. */
+pk_status pk_kernel_ctc_beam(int device, int n_utt, const int32_t *row_off, int rows, int V, const float *logprobs, int width,
+                             const pk_lm *lm, const pk_vocab *vocab, float alpha, float beta, int cap, int32_t *tok, int32_t *t_start,
+                             int32_t *t_end, float *t_conf, int32_t *topk_id, float *topk_lp, float *blank_lp, int32_t *bp,
+                             int64_t *guard_bad);
 
 /* Offline speaker diarization: Sortformer (include/parakeet/sortformer.hpp, src/sortformer.cpp:42-122 of the reference).
  * PCM -> log-mel WITHOUT per-bin normalisation (main.cpp:514-517) -> NEST encoder (the offline FastConformer under keys

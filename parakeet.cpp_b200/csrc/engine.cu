@@ -794,6 +794,30 @@ pk_status pk_engine::run_ctc(float *logprobs_dev) {
     return PK_OK;
 }
 
+// PK_DECODER_CTC_BEAM: the CTC head and frame pass as run_ctc (log-probs into the idle qkv workspace), then the per-frame
+// top-W over every frame of the batch and the beam search, one CTA per utterance (ctc_beam.cu).
+pk_status pk_engine::run_ctc_beam() {
+    const pk_config &c = cfg;
+    if ((size_t)M * c.vocab > (size_t)Bmax * Tmax * 3 * c.d_model) return fail(PK_ERR_CAPACITY, "CTC beam search: workspace too small for the log-probs");
+    const int ldv = (c.vocab + 3) & ~3;
+    EpiParams ep;
+    ep.kind = EPI_BIAS_F32;
+    ep.out_f32 = logits;
+    ep.ldo = ldv;
+    gemm(enc_operand(this), c.d_model, ctc_head, M, ep);
+    {
+        Scope sc(this, CAT_CTC);
+        launch_ctc_frame_argmax(logits, M, c.vocab, ldv, best, bconf, qkv, stream);
+        launch_ctc_frame_topk(qkv, M, c.vocab, beam_w, beam_topk_id, beam_topk_lp, beam_blank, stream);
+        launch_ctc_beam(qkv, beam_topk_id, beam_topk_lp, beam_blank, d_row_off, n_utt, c.vocab, beam_w, cap, beam_lm, beam_pc, beam_bp,
+                        tok, t_start, t_end, t_conf, stream);
+    }
+    launches += 3;
+    last_tdt = false;
+    PK_CUDA(cudaGetLastError());
+    return PK_OK;
+}
+
 pk_status pk_engine::run_tdt() {
     const pk_config &c = cfg;
     // enc_proj for all frames at once (joint's first Linear, tdt.cpp:17)
@@ -1131,6 +1155,7 @@ void pk_engine_destroy(pk_engine *e) {
     cudaSetDevice(e->device);
     if (e->stream) cudaStreamSynchronize(e->stream);
     for (void *p : e->allocs) cudaFree(p);
+    for (void *p : e->beam_tab) cudaFree(p);
     for (auto &kv : e->graphs)
         if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
     for (auto &r : e->prof) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
@@ -1691,6 +1716,12 @@ static pk_status run_front(pk_engine *e) {
 // (a model without a CTC head rejects PK_DECODER_CTC in run_ctc).
 static pk_status check_decoder(pk_engine *e, pk_decoder dec) {
     if (e->diar) return e->fail(PK_ERR_INVALID, "a Sortformer engine has no decoder: use pk_sortformer_forward / pk_diarize_batch");
+    if (dec == PK_DECODER_CTC_BEAM) {
+        if (!e->cfg.has_ctc) return e->fail(PK_ERR_INVALID, "PK_DECODER_CTC_BEAM: this model has no CTC head");
+        if (!e->beam_w) return e->fail(PK_ERR_INVALID, "PK_DECODER_CTC_BEAM: call pk_set_ctc_beam first");
+        if (e->boosting()) return e->fail(PK_ERR_INVALID, "PK_DECODER_CTC_BEAM: phrase boosting is set (beam search does not boost)");
+        return PK_OK;
+    }
     const bool rnnt_model = e->cfg.n_durations == 0;
     if (dec == PK_DECODER_TDT && rnnt_model)
         return e->fail(PK_ERR_INVALID, "PK_DECODER_TDT on an RNN-T model (n_durations = 0): use PK_DECODER_RNNT");
@@ -1701,7 +1732,7 @@ static pk_status check_decoder(pk_engine *e, pk_decoder dec) {
 static pk_status run_pipeline(pk_engine *e, pk_decoder dec) {   // everything after the front end
     pk_status s;
     if ((s = e->run_encoder(nullptr, nullptr))) return s;
-    return dec == PK_DECODER_CTC ? e->run_ctc(nullptr) : e->run_tdt();
+    return e->run_decoder(dec);
 }
 
 // The ~250 launches of one batch are replayed as ONE CUDA graph once a batch shape has been seen
@@ -1721,7 +1752,13 @@ pk_status pk_run_staged(pk_engine *e, pk_decoder dec) {
 }
 
 static pk_status run_asr_graph(pk_engine *e, pk_decoder dec) {
-    std::string key(1, dec == PK_DECODER_CTC ? 'c' : (dec == PK_DECODER_RNNT ? 'r' : 't'));
+    std::string key(1, dec == PK_DECODER_CTC ? 'c' : (dec == PK_DECODER_RNNT ? 'r' : (dec == PK_DECODER_CTC_BEAM ? 'B' : 't')));
+    if (dec == PK_DECODER_CTC_BEAM) {                   // width, tables, weights: pk_set_ctc_beam drops the 'B' graphs of old tables
+        const int32_t wg[2] = {e->beam_w, e->beam_gen};
+        const double ab[2] = {e->beam_lm.alpha_ln10, e->beam_lm.beta};
+        key.append(reinterpret_cast<const char *>(wg), sizeof(wg));
+        key.append(reinterpret_cast<const char *>(ab), sizeof(ab));
+    }
     // (per-row lists live in buffers that never move: one graph serves every set of lists)
     const int32_t bg = e->brows_on ? -1 : (e->boost_on ? e->boost_gen : 0);
     key.append(reinterpret_cast<const char *>(&bg), sizeof(bg));
@@ -2035,6 +2072,68 @@ pk_status pk_engine::boost_upload(const char *fn, BoostSlots &dst, int row0, int
     return PK_OK;
 }
 
+pk_status pk_set_ctc_beam(pk_engine *e, int32_t width, const pk_lm *lm, const pk_vocab *vocab, float alpha, float beta) {
+    if (!e) return PK_ERR_INVALID;
+    if (e->diar) return e->fail(PK_ERR_INVALID, "pk_set_ctc_beam: a Sortformer engine has no decoder");
+    if (!e->cfg.has_ctc) return e->fail(PK_ERR_INVALID, "pk_set_ctc_beam: this model has no CTC head");
+    if (width < 1 || width > PK_CTC_BEAM_MAX)
+        return e->fail(PK_ERR_INVALID, "pk_set_ctc_beam: width " + std::to_string(width) + " (1.." + std::to_string(PK_CTC_BEAM_MAX) + ")");
+    if (lm && !vocab) return e->fail(PK_ERR_INVALID, "pk_set_ctc_beam: a language model needs the vocabulary");
+    if (!std::isfinite(alpha) || !std::isfinite(beta)) return e->fail(PK_ERR_INVALID, "pk_set_ctc_beam: alpha and beta must be finite");
+    cudaSetDevice(e->device);
+    if (!e->beam_bp) {
+        const size_t rows = (size_t)e->Bmax * e->Tmax;
+        e->beam_topk_id = e->dalloc<int32_t>(rows * PK_CTC_BEAM_MAX);
+        e->beam_bp = e->dalloc<int32_t>(rows * PK_CTC_BEAM_MAX);
+        e->beam_topk_lp = e->dalloc<float>(rows * PK_CTC_BEAM_MAX);
+        e->beam_blank = e->dalloc<float>(rows);
+        if (!e->beam_topk_id || !e->beam_bp || !e->beam_topk_lp || !e->beam_blank) {
+            e->beam_bp = nullptr;
+            return e->fail(PK_ERR_CUDA, "cudaMalloc failed (beam-search workspace)");
+        }
+    }
+    // The tables are uploaded only when the LM or the vocabulary changes; a call that only repeats them (one per request)
+    // costs nothing and keeps the captured graphs.  A replacement first drops the graphs that read the old tables, then
+    // frees them.
+    const uint64_t id = ctc_beam_tables_id(lm, vocab, e->cfg.vocab);
+    if (id != e->beam_tab_id) {
+        cudaStreamSynchronize(e->stream);
+        for (auto it = e->graphs.begin(); it != e->graphs.end();) {
+            if (it->first[0] != 'B') { ++it; continue; }
+            if (it->second.exec) cudaGraphExecDestroy(it->second.exec);
+            it = e->graphs.erase(it);
+        }
+        for (void *p : e->beam_tab) cudaFree(p);
+        e->beam_tab.clear();
+        e->beam_lm = DeviceLM{};
+        e->beam_pc = DevicePieces{};
+        e->beam_tab_id = 0;
+        e->beam_w = 0;
+        ++e->beam_gen;
+        DeviceLM dlm;
+        DevicePieces dpc;
+        const std::string msg = ctc_beam_tables(lm, vocab, e->cfg.vocab, [e](const void *h, size_t bytes) -> void * {
+            void *d = nullptr;
+            if (cudaMalloc(&d, std::max<size_t>(bytes, 1)) != cudaSuccess) return nullptr;
+            e->beam_tab.push_back(d);
+            if (bytes && (cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, e->stream) != cudaSuccess ||
+                          cudaStreamSynchronize(e->stream) != cudaSuccess)) return nullptr;
+            return d;
+        }, &dlm, &dpc);
+        if (!msg.empty()) {
+            for (void *p : e->beam_tab) cudaFree(p);
+            e->beam_tab.clear();
+            return e->fail(msg.rfind("cudaMalloc", 0) == 0 ? PK_ERR_CUDA : PK_ERR_INVALID, "pk_set_ctc_beam: " + msg);
+        }
+        e->beam_lm = dlm;
+        e->beam_pc = dpc;
+        e->beam_tab_id = id;
+    }
+    e->beam_lm.set_weights(alpha, beta);
+    e->beam_w = width;
+    return PK_OK;
+}
+
 pk_status pk_set_boost(pk_engine *e, const int32_t *phrase_ids, const int32_t *phrase_off, int32_t n_phrases, float boost) {
     if (!e || n_phrases < 0 || (n_phrases > 0 && (!phrase_ids || !phrase_off))) return PK_ERR_INVALID;
     if (e->diar) return e->fail(PK_ERR_INVALID, "pk_set_boost: a Sortformer engine has no decoder");
@@ -2189,7 +2288,7 @@ pk_status pk_decode(pk_engine *e, const float *enc, const int32_t *enc_lens, int
     pk_status s;
     if ((s = check_decoder(e, dec))) return s;
     if ((s = stage_enc(e, enc, enc_lens, n_utt))) return s;
-    if ((s = (dec == PK_DECODER_CTC ? e->run_ctc(nullptr) : e->run_tdt()))) return s;
+    if ((s = e->run_decoder(dec))) return s;
     return e->fetch(out);
 }
 

@@ -214,6 +214,17 @@ struct pk_engine {
     bool boosting() const { return boost_on || brows_on; }
     DeviceTrie boost_trie() const { return brows_on ? brows.trie() : trie; }
 
+    // ---- CTC beam search (pk_set_ctc_beam)
+    int beam_w = 0;                                    // 0: not set
+    int beam_gen = 0;                                  // bumps when the device tables are replaced (part of the CUDA-graph key)
+    uint64_t beam_tab_id = 0;                          // ctc_beam_tables_id of the tables on the device (0: no LM)
+    std::vector<void *> beam_tab;                      // their device buffers, freed when they are replaced
+    DeviceLM beam_lm{};
+    DevicePieces beam_pc{};
+    // [Bmax Tmax][PK_CTC_BEAM_MAX] top-W ids / log-probs and back-pointers, [Bmax Tmax] blank log-probs (allocated once)
+    int32_t *beam_topk_id = nullptr, *beam_bp = nullptr;
+    float *beam_topk_lp = nullptr, *beam_blank = nullptr;
+
     // ---- optional per-kernel-class timing (CUDA events on the engine stream)
     enum { CAT_MEL, CAT_SUBSAMPLE, CAT_GEMM, CAT_LAYERNORM, CAT_ATTENTION, CAT_DWCONV, CAT_CTC, CAT_TDT, CAT_MHA, CAT_HEAD, CAT_N };
     struct ProfRec { int cat; cudaEvent_t a, b; double flops; };
@@ -310,6 +321,10 @@ struct pk_engine {
     pk_status run_stream_decode();
     pk_status run_ctc(float *logprobs_dev_or_null);
     pk_status run_tdt();
+    pk_status run_ctc_beam();
+    pk_status run_decoder(pk_decoder dec) {           // (dec already checked)
+        return dec == PK_DECODER_CTC ? run_ctc(nullptr) : (dec == PK_DECODER_CTC_BEAM ? run_ctc_beam() : run_tdt());
+    }
     pk_status fetch(pk_tokens *out);
 };
 

@@ -711,3 +711,40 @@ pk_status pk_kernel_speaker_head(int device, int M, int D, int S, const float *x
 }
 
 }  // extern "C"
+
+extern "C" pk_status pk_kernel_ctc_beam(int device, int n_utt, const int32_t *row_off, int rows, int V, const float *logprobs, int width,
+                                        const pk_lm *lm, const pk_vocab *vocab, float alpha, float beta, int cap, int32_t *tok,
+                                        int32_t *t_start, int32_t *t_end, float *t_conf, int32_t *topk_id, float *topk_lp, float *blank_lp,
+                                        int32_t *bp, int64_t *guard_bad) {
+    if (V < 2 || rows < 0 || width < 1 || width > PK_CTC_BEAM_MAX || cap < 1 || !tok || (rows > 0 && !logprobs) ||
+        !offsets_ok(row_off, n_utt, rows) || (lm && !vocab))
+        return PK_ERR_INVALID;
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const size_t R = std::max(rows, 1);
+    const float *dlp = cx.upload(logprobs, (size_t)rows * V);
+    const int32_t *doff = cx.upload(row_off, (size_t)n_utt + 1);
+    int32_t *dtok = cx.guarded<int32_t>((size_t)n_utt * (1 + cap));
+    int32_t *dst = cx.guarded<int32_t>((size_t)n_utt * cap), *den = cx.guarded<int32_t>((size_t)n_utt * cap);
+    float *dcf = cx.guarded<float>((size_t)n_utt * cap);
+    int32_t *did = cx.guarded<int32_t>(R * width), *dbp = cx.guarded<int32_t>(R * width);
+    float *dtl = cx.guarded<float>(R * width), *dbl = cx.guarded<float>(R);
+    if (!cx.ok) return PK_ERR_CUDA;
+    DeviceLM dlm;
+    DevicePieces dpc;
+    const std::string msg = ctc_beam_tables(lm, vocab, V, [&cx](const void *h, size_t bytes) -> void * {
+        return cx.upload(static_cast<const uint8_t *>(h), bytes);
+    }, &dlm, &dpc);
+    dlm.set_weights(alpha, beta);
+    if (!msg.empty() || !cx.ok) return msg.empty() || msg.rfind("cudaMalloc", 0) == 0 ? PK_ERR_CUDA : PK_ERR_INVALID;
+    launch_ctc_frame_topk(dlp, rows, V, width, did, dtl, dbl, cx.st);
+    launch_ctc_beam(dlp, did, dtl, dbl, doff, n_utt, V, width, cap, dlm, dpc, dbp, dtok, dst, den, dcf, cx.st);
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    auto get_i = [](int32_t *h, const int32_t *d, size_t n) { return !h || cudaMemcpy(h, d, n * 4, cudaMemcpyDeviceToHost) == cudaSuccess; };
+    if (!get_i(tok, dtok, (size_t)n_utt * (1 + cap)) || !get_i(t_start, dst, (size_t)n_utt * cap) || !get_i(t_end, den, (size_t)n_utt * cap) ||
+        !fetch_f32(t_conf, dcf, (size_t)n_utt * cap) || !get_i(topk_id, did, (size_t)rows * width) || !fetch_f32(topk_lp, dtl, (size_t)rows * width) ||
+        !fetch_f32(blank_lp, dbl, rows) || !get_i(bp, dbp, (size_t)rows * width))
+        return PK_ERR_CUDA;
+    return PK_OK;
+}

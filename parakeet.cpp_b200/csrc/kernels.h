@@ -2,11 +2,16 @@
 #pragma once
 #include <cuda.h>
 
+#include <functional>
+#include <string>
 #include <vector>
 
 #include "pk_common.cuh"
 
 #define PK_MAX_LSTM 4
+
+struct pk_lm;
+struct pk_vocab;
 
 namespace pk {
 
@@ -223,6 +228,50 @@ void launch_ctc_frame_argmax(const float *logits, int M, int V, int ld, int32_t 
                              float *logprobs, cudaStream_t st);
 void launch_ctc_collapse(const int32_t *best, const float *conf, const int32_t *row_off, int n_utt, int blank,
                          int cap, int32_t *tok, int32_t *t_start, int32_t *t_end, float *t_conf, cudaStream_t st);
+
+// ------------------------------------------------------------------ ctc_beam.cu (CTC prefix beam search, DESIGN.md section 14)
+// Word n-gram LM in open-addressing tables (built on the host by lm.cpp): words by 64-bit FNV-1a hash of their bytes,
+// n-grams by (context entry + 1) << 32 | word id.  Entry 0 is the empty context; an entry's suffix is its longest present
+// proper suffix.  Empty slots hold key 0.  word_key == nullptr: no LM.
+struct DeviceLM {
+    const unsigned long long *word_key = nullptr;
+    const int32_t *word_id = nullptr;
+    const unsigned long long *ng_key = nullptr;
+    const int32_t *ng_val = nullptr;
+    const double *prob = nullptr, *backoff = nullptr;   // log10
+    const int32_t *suffix = nullptr, *order = nullptr;
+    uint32_t word_mask = 0, ng_mask = 0;
+    int32_t max_order = 0, start = 0, unk = 0, eos = 0;
+    double alpha_ln10 = 0.0, beta = 0.0;
+    void set_weights(float alpha, float beta_) {
+        alpha_ln10 = (double)alpha * 2.302585092994045684;
+        beta = (double)beta_;
+    }
+};
+// Token pieces for word boundaries: the bytes of token v are bytes[off[v] .. off[v+1]) with a leading U+2581 removed;
+// starts[v] = 1 when the piece began with it.
+struct DevicePieces {
+    const uint8_t *bytes = nullptr;
+    const int32_t *off = nullptr;
+    const uint8_t *starts = nullptr;
+};
+constexpr int CTC_BEAM_THREADS = 256;
+// Per frame: the `width` best non-blank (id, log-prob) pairs, ties to the lower id, into topk_id / topk_lp [M][width]
+// (id -1 = absent: fewer than `width` finite values), and lp[blank] into blank_lp [M].
+void launch_ctc_frame_topk(const float *logprobs, int M, int V, int width, int32_t *topk_id, float *topk_lp, float *blank_lp,
+                           cudaStream_t st);
+// The device form of an LM (or none: lm == NULL) and of the vocabulary's pieces; the weights are set by
+// DeviceLM::set_weights.  Every table goes through upload(host, bytes) -> device pointer (nullptr: out of memory).  Returns
+// an error message, empty on success.
+std::string ctc_beam_tables(const pk_lm *lm, const pk_vocab *vocab, int V, const std::function<void *(const void *, size_t)> &upload,
+                            DeviceLM *lm_out, DevicePieces *pc_out);
+// What the tables of ctc_beam_tables(lm, vocab, V) are made from: 0 without an LM, else a 64-bit identity of the LM
+// object (each pk_lm_load gives a new one) and of the vocabulary's first V - 1 pieces.
+uint64_t ctc_beam_tables_id(const pk_lm *lm, const pk_vocab *vocab, int V);
+// One CTA per utterance: the beam search over its frames; back-pointers bp [M][width]; tokens in the greedy layout.
+void launch_ctc_beam(const float *logprobs, const int32_t *topk_id, const float *topk_lp, const float *blank_lp,
+                     const int32_t *row_off, int n_utt, int V, int width, int cap, const DeviceLM &lm, const DevicePieces &pieces,
+                     int32_t *bp, int32_t *tok, int32_t *t_start, int32_t *t_end, float *t_conf, cudaStream_t st);
 
 // ------------------------------------------------------------------ tdt.cu (K10)
 struct TdtParams {

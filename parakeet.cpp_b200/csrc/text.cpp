@@ -21,10 +21,15 @@
 #include <vector>
 
 #include "../../include/parakeet_b200.h"
+#include "lm.h"
 
 struct pk_vocab {
     std::vector<std::string> pieces;
 };
+
+namespace pk {
+const std::vector<std::string> *vocab_pieces(const pk_vocab *v) { return v ? &v->pieces : nullptr; }
+}  // namespace pk
 
 namespace {
 const char kMark[] = "\xe2\x96\x81";  // U+2581

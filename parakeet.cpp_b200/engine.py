@@ -99,7 +99,8 @@ EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_co
            "pk_fetch_probs", "pk_diar_segments", "pk_kernel_mha", "pk_kernel_speaker_head",
            "pk_diar_stream_open", "pk_diar_stream_reset", "pk_diar_stream_step", "pk_diar_stream_step_feats", "pk_diar_stream_speakers",
            "pk_diar_stream_count", "pk_set_boost_rows", "pk_stream_set_boost", "pk_kernel_tdt_decode_boosted",
-           "pk_transcribe_diarize_batch", "pk_run_transcribe_diarize_staged", "pk_diarize_transcription", "pk_diarize_words"]
+           "pk_transcribe_diarize_batch", "pk_run_transcribe_diarize_staged", "pk_diarize_transcription", "pk_diarize_words",
+           "pk_lm_load", "pk_lm_free", "pk_lm_order", "pk_lm_count", "pk_lm_sentence_log10", "pk_set_ctc_beam", "pk_kernel_ctc_beam"]
 
 _lib = None
 
@@ -215,6 +216,17 @@ def load_library():
     L.pk_diarize_transcription.argtypes = [f32p, f32p, C.c_int32, i32p, f32p, f32p, C.c_int32, i32p]
     L.pk_diarize_words.argtypes = [f32p, C.c_int32, C.c_int32, C.c_float, f32p, f32p, C.c_int32, i32p, i32p, f32p, f32p, C.c_int32]
     L.pk_diarize_words.restype = C.c_int32
+    L.pk_lm_load.argtypes = [C.c_char_p, C.POINTER(vp)]
+    L.pk_lm_free.argtypes = [vp]
+    L.pk_lm_order.argtypes = [vp]
+    L.pk_lm_order.restype = C.c_int32
+    L.pk_lm_count.argtypes = [vp, C.c_int32]
+    L.pk_lm_count.restype = C.c_int64
+    L.pk_lm_sentence_log10.argtypes = [vp, C.c_char_p]
+    L.pk_lm_sentence_log10.restype = C.c_double
+    L.pk_set_ctc_beam.argtypes = [vp, C.c_int32, vp, vp, C.c_float, C.c_float]
+    L.pk_kernel_ctc_beam.argtypes = [C.c_int, C.c_int, i32p, C.c_int, C.c_int, f32p, C.c_int, vp, vp, C.c_float, C.c_float, C.c_int,
+                                     i32p, i32p, i32p, f32p, i32p, f32p, f32p, i32p, i64p]
     _lib = L
     return L
 
@@ -447,6 +459,7 @@ class Decoder(enum.IntEnum):          # transcribe.hpp:34
     CTC = 0
     TDT = 1
     RNNT = 2
+    CTC_BEAM = 3                      # CTC prefix beam search (Engine.set_ctc_beam; DESIGN.md section 14)
 
 
 @dataclass
@@ -860,6 +873,13 @@ class Engine:
         ids, off, _ = pack_phrase_lists([phrases])
         self._check(self.L.pk_stream_set_boost(self.h, stream, _i32p(ids), _i32p(off), len(phrases), float(boost)), "pk_stream_set_boost")
 
+    def set_ctc_beam(self, width: int, lm: Optional["LanguageModel"] = None, vocab=None, alpha: float = 0.5, beta: float = 1.0):
+        """Beam width and optional word n-gram LM for Decoder.CTC_BEAM (pk_set_ctc_beam).  vocab: a Tokenizer or a vocab
+        path, needed with an LM (word boundaries come from its pieces)."""
+        tok = Tokenizer(vocab) if isinstance(vocab, str) else vocab
+        self._check(self.L.pk_set_ctc_beam(self.h, int(width), lm.h if lm is not None else None, tok.h if tok is not None else None,
+                                           float(alpha), float(beta)), "pk_set_ctc_beam")
+
     # -- non-16 kHz input: converted on the device (SURVEY.md section 8f row 4)
     def stage_rate(self, pcms: Sequence[np.ndarray], src_rate: int):
         buf, off = _pack(pcms)
@@ -962,6 +982,38 @@ def pack_phrase_lists(lists):
     row = np.zeros(len(lists) + 1, np.int32)
     row[1:] = np.cumsum([len(lst) for lst in lists])
     return ids, off, row
+
+
+class LanguageModel:
+    """A word n-gram LM read from an ARPA file (pk_lm_load), for Engine.set_ctc_beam."""
+
+    def __init__(self, arpa_path: str):
+        self.L = load_library()
+        self.h = C.c_void_p()
+        if self.L.pk_lm_load(arpa_path.encode(), C.byref(self.h)) != 0:
+            raise RuntimeError("pk_lm_load: " + self.L.pk_last_error(None).decode())
+
+    @property
+    def order(self) -> int:
+        return self.L.pk_lm_order(self.h)
+
+    def count(self, order: int) -> int:
+        return self.L.pk_lm_count(self.h, order)
+
+    def sentence_log10(self, words: str) -> float:
+        """log10 p(words </s> | <s>) by ARPA back-off."""
+        return self.L.pk_lm_sentence_log10(self.h, words.encode("utf-8"))
+
+    def close(self):
+        if self.h:
+            self.L.pk_lm_free(self.h)
+            self.h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class Tokenizer:
