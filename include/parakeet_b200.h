@@ -299,6 +299,27 @@ pk_status pk_kernel_dwconv(int device, int math, int n_utt, const int32_t *row_o
 /* CTC head reduction of logits [M][ld]: best [M] (first maximum), conf [M] = exp(max log-prob), logprobs [M][V] (or NULL). */
 pk_status pk_kernel_ctc_argmax(int device, int M, int V, int ld, const float *logits, int32_t *best, float *conf, float *logprobs,
                                int64_t *guard_bad);
+/* The front end.  pk_kernel_mel: the offline log-mel (and, with normalize = 1, the per-utterance normalisation) of utterances
+ * b = pcm[pcm_off[b] .. pcm_off[b+1]) (n >= 400 samples with normalize = 1, >= 2 without), 1 + n / 160 frames each, packed:
+ * logmel_out [frames][n_mels] (with normalize = 0 the kernel's only output) and feats_out [frames][n_mels] (NULL with
+ * normalize = 0).  n_mels a multiple of 8 up to 640.  pk_kernel_mel_stream: the streaming log-mel of already pre-emphasised
+ * signals b = sig[sig_off[b] .. sig_off[b+1]), n_frames[b] frames (frame f reads samples 160 f .. 160 f + 511) into rows
+ * out_row[b] + f of logmel_out [rows_total][n_mels]; the other rows are not written. */
+pk_status pk_kernel_mel(int device, int n_utt, const int64_t *pcm_off, const float *pcm, int n_mels, int normalize, float *logmel_out,
+                        float *feats_out, int64_t *guard_bad);
+pk_status pk_kernel_mel_stream(int device, int n_streams, const int64_t *sig_off, const float *sig, const int32_t *n_frames,
+                               const int32_t *out_row, int rows_total, int n_mels, float *logmel_out, int64_t *guard_bad);
+/* The convolutional front of the subsampling (3x3 kernels, stride 2, zero padding 1; weights [C][9] unless noted).
+ * pk_kernel_subsample_conv1: conv1_ (1 -> C) + ReLU + depthwise dw1_ of utterances b = feature rows [frame_off[b], frame_off[b+1])
+ * of feats [rows_total][mel] (mel even, C a multiple of 4 up to 1024) -> rows (t2, f2) per utterance, packed, of C channels.
+ * pk_kernel_subsample_dw: depthwise dw2_ (tap-major weights [9][C]) of utterances of in_rows[b] x fin rows of C channels
+ * packed in `in` -> conv_len(in_rows[b]) x conv_len(fin) rows each, packed.  Output: out_f32 with PK_MATH_FP32, else hi and,
+ * with PK_MATH_BF16X3, lo (the engine's activation operand). */
+pk_status pk_kernel_subsample_conv1(int device, int math, int n_utt, const int32_t *frame_off, int rows_total, const float *feats, int mel,
+                                    int C, const float *w1, const float *b1, const float *wd, const float *bd, float *out_f32, float *hi,
+                                    float *lo, int64_t *guard_bad);
+pk_status pk_kernel_subsample_dw(int device, int math, int n_utt, const int32_t *in_rows, int fin, int C, const float *in, const float *wd_tapmajor,
+                                 const float *bd, float *out_f32, float *hi, float *lo, int64_t *guard_bad);
 
 /* The TDT / RNN-T decode kernel (csrc/tdt.cu) on host fp32 inputs in the reference's layouts, with the TdtParams that the engine
  * builds: Bpad = n_utt rounded up to 32, LSTM weights reordered unit-major and split into bf16 hi/lo rows, the initial h split into

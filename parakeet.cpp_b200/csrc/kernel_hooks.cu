@@ -748,3 +748,147 @@ extern "C" pk_status pk_kernel_ctc_beam(int device, int n_utt, const int32_t *ro
         return PK_ERR_CUDA;
     return PK_OK;
 }
+
+namespace {
+
+int conv_len3(int n) { return (n - 1) / 2 + 1; }   // 3 taps, stride 2, padding 1
+
+// the engine's mel tables, uploaded into the hook's buffers
+MelTables hook_mel_tables(HookCtx &cx, int n_mels) {
+    return build_mel_tables(n_mels, [&cx](const void *h, size_t bytes) -> void * {
+        return cx.upload(static_cast<const uint8_t *>(h), bytes);
+    });
+}
+
+bool mel_bins_ok(int n_mels) { return n_mels >= 8 && n_mels <= MEL_NORM_THREADS && n_mels % 8 == 0; }
+
+}  // namespace
+
+extern "C" {
+
+// K1 (+ K2) as pk_engine::run_mel launches them.  Utterance b = pcm[pcm_off[b] .. pcm_off[b+1]) (samples before pcm_off[0]
+// are uploaded too and must not be read); frame_off as the engine derives it (1 + n / 160 frames each).  normalize = 1:
+// logmel_out = the intermediate log-mel, feats_out = the normalised features; normalize = 0 (Sortformer): logmel_out = the
+// log-mel the kernel writes into the engine's feature buffer, feats_out = NULL.
+pk_status pk_kernel_mel(int device, int n_utt, const int64_t *pcm_off, const float *pcm, int n_mels, int normalize, float *logmel_out,
+                        float *feats_out, int64_t *guard_bad) {
+    if (n_utt < 1 || !pcm_off || !pcm || pcm_off[0] < 0 || !mel_bins_ok(n_mels) || !logmel_out || (normalize != 0) != (feats_out != nullptr))
+        return PK_ERR_INVALID;
+    std::vector<int32_t> frame_off(n_utt + 1, 0);
+    int maxF = 0;
+    for (int b = 0; b < n_utt; ++b) {
+        const int64_t n = pcm_off[b + 1] - pcm_off[b];
+        if (n < (normalize ? 400 : 2) || n > ((int64_t)1 << 30)) return PK_ERR_INVALID;
+        const int F = (int)(1 + n / 160);
+        frame_off[b + 1] = frame_off[b] + F;
+        maxF = std::max(maxF, F);
+    }
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const size_t n_o = (size_t)frame_off[n_utt] * n_mels;
+    const MelTables tb = hook_mel_tables(cx, n_mels);
+    int64_t *doff = cx.upload(pcm_off, n_utt + 1);
+    int32_t *dfo = cx.upload(frame_off.data(), n_utt + 1);
+    float *dpcm = cx.upload(pcm, (size_t)pcm_off[n_utt]);
+    float *lm = cx.guarded<float>(n_o), *ft = normalize ? cx.guarded<float>(n_o) : nullptr;
+    float *part = normalize ? static_cast<float *>(cx.alloc(mel_part_floats(n_utt, n_mels) * sizeof(float))) : nullptr;
+    if (!cx.ok) return PK_ERR_CUDA;
+    if (normalize) launch_mel(dpcm, doff, dfo, n_utt, maxF, n_mels, tb, lm, ft, part, cx.st, true);
+    else launch_mel(dpcm, doff, dfo, n_utt, maxF, n_mels, tb, nullptr, lm, nullptr, cx.st, false);
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    return fetch_f32(logmel_out, lm, n_o) && (!ft || fetch_f32(feats_out, ft, n_o)) ? PK_OK : PK_ERR_CUDA;
+}
+
+// The streaming K1 as pk_stream_step launches it: stream b's pre-emphasised signal sig[sig_off[b] .. sig_off[b+1]) gives
+// n_frames[b] frames (frame f reads samples f * 160 .. f * 160 + 511) into rows out_row[b] + f of logmel_out [rows_total][n_mels].
+pk_status pk_kernel_mel_stream(int device, int n_streams, const int64_t *sig_off, const float *sig, const int32_t *n_frames,
+                               const int32_t *out_row, int rows_total, int n_mels, float *logmel_out, int64_t *guard_bad) {
+    if (n_streams < 1 || !sig_off || !sig || !n_frames || !out_row || rows_total < 1 || sig_off[0] < 0 || !mel_bins_ok(n_mels) || !logmel_out)
+        return PK_ERR_INVALID;
+    int maxF = 0;
+    for (int b = 0; b < n_streams; ++b) {
+        const int64_t n = sig_off[b + 1] - sig_off[b];
+        if (n < 0 || n_frames[b] < 0 || out_row[b] < 0 || (int64_t)out_row[b] + n_frames[b] > rows_total) return PK_ERR_INVALID;
+        if (n_frames[b] > 0 && (int64_t)(n_frames[b] - 1) * 160 + 512 > n) return PK_ERR_INVALID;
+        maxF = std::max(maxF, n_frames[b]);
+    }
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const size_t n_o = (size_t)rows_total * n_mels;
+    const MelTables tb = hook_mel_tables(cx, n_mels);
+    int64_t *doff = cx.upload(sig_off, n_streams + 1);
+    int32_t *dnf = cx.upload(n_frames, n_streams), *drow = cx.upload(out_row, n_streams);
+    float *dsig = cx.upload(sig, (size_t)sig_off[n_streams]);
+    float *lm = cx.guarded<float>(n_o);
+    if (!cx.ok) return PK_ERR_CUDA;
+    launch_mel_stream(dsig, doff, dnf, drow, n_streams, maxF, n_mels, tb, lm, cx.st);
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    return fetch_f32(logmel_out, lm, n_o) ? PK_OK : PK_ERR_CUDA;
+}
+
+// K3 (conv1 + ReLU + dw1) as pk_engine::run_conv1 launches it: utterance b = feature rows [frame_off[b], frame_off[b+1]) of
+// feats [rows_total][mel] (other rows may exist and must not be read); weights [C][9] as stored.  Output rows
+// (s2_off[b] + t2) * f2n + f2 of C channels, s2_off as the engine derives it, in sub1's form for `math`: out_f32, or hi and,
+// with PK_MATH_BF16X3, lo.
+pk_status pk_kernel_subsample_conv1(int device, int math, int n_utt, const int32_t *frame_off, int rows_total, const float *feats, int mel,
+                                    int C, const float *w1, const float *b1, const float *wd, const float *bd, float *out_f32, float *hi,
+                                    float *lo, int64_t *guard_bad) {
+    if (!offsets_ok(frame_off, n_utt, rows_total) || mel < 2 || mel % 2 || mel > MEL_NORM_THREADS || C < 4 || C % 4 || C > 1024 || !feats ||
+        !w1 || !b1 || !wd || !bd || !act_out_ok(math, out_f32, hi, lo))
+        return PK_ERR_INVALID;
+    std::vector<int32_t> s2_off(n_utt + 1, 0);
+    int maxT2 = 0;
+    for (int b = 0; b < n_utt; ++b) {
+        const int F = frame_off[b + 1] - frame_off[b];
+        if (F < 1) return PK_ERR_INVALID;
+        const int t2 = conv_len3(conv_len3(F));
+        s2_off[b + 1] = s2_off[b] + t2;
+        maxT2 = std::max(maxT2, t2);
+    }
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const size_t n_o = (size_t)s2_off[n_utt] * conv_len3(conv_len3(mel)) * C;
+    int32_t *dfo = cx.upload(frame_off, n_utt + 1), *ds2 = cx.upload(s2_off.data(), n_utt + 1);
+    float *df = cx.upload(feats, (size_t)rows_total * mel);
+    float *dw1 = cx.upload(w1, (size_t)C * 9), *db1 = cx.upload(b1, C), *dwd = cx.upload(wd, (size_t)C * 9), *dbd = cx.upload(bd, C);
+    ActBuf out = guarded_act(cx, math, n_o, lo != nullptr);
+    if (!cx.ok) return PK_ERR_CUDA;
+    launch_subsample_conv1_dw1(df, dfo, ds2, n_utt, maxT2, mel, C, dw1, db1, dwd, dbd, out, cx.st);
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    return fetch_act(out, out_f32, hi, lo, n_o) ? PK_OK : PK_ERR_CUDA;
+}
+
+// K4 (depthwise 3x3, stride 2, padding 1 on channels-last rows) as pk_engine::run_subsample_tail launches it for dw2_:
+// utterance b has in_rows[b] time rows of fin frequency rows of C channels, packed in order in `in`; its output has
+// conv_len(in_rows[b]) x conv_len(fin) rows, packed in the same order.  wd tap-major [9][C] (as dw2_wt), bd [C].  Output in
+// sub3's form for `math`.
+pk_status pk_kernel_subsample_dw(int device, int math, int n_utt, const int32_t *in_rows, int fin, int C, const float *in, const float *wd_tapmajor,
+                                 const float *bd, float *out_f32, float *hi, float *lo, int64_t *guard_bad) {
+    if (n_utt < 1 || !in_rows || fin < 1 || C < 4 || C % 4 || !in || !wd_tapmajor || !bd || !act_out_ok(math, out_f32, hi, lo))
+        return PK_ERR_INVALID;
+    std::vector<int32_t> in_off(n_utt + 1, 0), out_off(n_utt + 1, 0);
+    for (int b = 0; b < n_utt; ++b) {
+        if (in_rows[b] < 1 || (int64_t)in_off[b] + in_rows[b] > INT32_MAX) return PK_ERR_INVALID;
+        in_off[b + 1] = in_off[b] + in_rows[b];
+        out_off[b + 1] = out_off[b] + conv_len3(in_rows[b]);
+    }
+    const int fout = conv_len3(fin);
+    const int64_t out_rows = (int64_t)out_off[n_utt] * fout;
+    if (out_rows > INT32_MAX) return PK_ERR_INVALID;
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const size_t n_o = (size_t)out_rows * C;
+    int32_t *drows = cx.upload(in_rows, n_utt), *din = cx.upload(in_off.data(), n_utt + 1), *dout = cx.upload(out_off.data(), n_utt + 1);
+    float *dx = cx.upload(in, (size_t)in_off[n_utt] * fin * C), *dw = cx.upload(wd_tapmajor, (size_t)9 * C), *db = cx.upload(bd, C);
+    ActBuf out = guarded_act(cx, math, n_o, lo != nullptr);
+    if (!cx.ok) return PK_ERR_CUDA;
+    launch_subsample_dw(dx, drows, din, dout, n_utt, fin, C, dw, db, out, (int)out_rows, cx.st);
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    return fetch_act(out, out_f32, hi, lo, n_o) ? PK_OK : PK_ERR_CUDA;
+}
+
+}  // extern "C"

@@ -24,6 +24,11 @@ struct MelTables {
     const int32_t *fb_start, *fb_len, *fb_off;   // [n_mels]
     int fb_nnz;
 };
+// The tables for n_mels bins, built on the host; every array goes through upload(host, bytes) -> device pointer
+// (nullptr: out of memory).
+MelTables build_mel_tables(int n_mels, const std::function<void *(const void *, size_t)> &upload);
+// K2 runs MEL_NORM_THREADS / n_mels frame groups of n_mels threads: the normalisation needs n_mels <= MEL_NORM_THREADS.
+constexpr int MEL_NORM_THREADS = 640;
 size_t mel_smem_bytes(const MelTables &tb);
 // part: scratch of mel_part_floats(n_utt, n_mels) floats (per-chunk statistics of the normalisation), one slice per utterance
 size_t mel_part_floats(int n_utt, int n_mels);

@@ -14,6 +14,8 @@
 //   once from DRAM; 4*n_mels bytes written per frame.
 // K2 mel_normalize_kernel: per utterance, per mel bin: mean, unbiased variance,
 //   (x - mean) / (sqrt(var) + 1e-5), two-pass like the reference.
+#include <cmath>
+
 #include "kernels.h"
 
 namespace pk {
@@ -195,7 +197,9 @@ mel_logpower_kernel(const float *__restrict__ pcm, const int64_t *__restrict__ p
 // utterance is cut into MEL_CH frame chunks: mel_stats_kernel reduces a chunk to (mean_c, M2_c = sum (x - mean_c)^2) per bin with
 // two sweeps over its own frames, mel_apply_kernel combines the MEL_CH partials of an utterance in a fixed order with Chan's
 // formula (mean = sum n_c mean_c / F, M2 = sum M2_c + n_c (mean_c - mean)^2: the accuracy of the two-pass form, deterministic,
-// independent of the batch) and normalises its chunk.  threads = (groups x n_mels).
+// independent of the batch) and normalises its chunk.  threads = (groups x n_mels).  Both work on x - x0, x0 = the bin's value in
+// the utterance's first frame: a constant bin (digital silence) then has chunk means and M2 of exactly 0 and comes out as 0,
+// where rounded means of the raw values would leave an offset of an ulp that 1 / (0 + 1e-5) scales up to O(1).
 constexpr int MEL_CH = 16;
 
 __device__ __forceinline__ void mel_chunk(int c, int F, int &f0, int &f1) {
@@ -217,10 +221,11 @@ __global__ void mel_stats_kernel(const float *__restrict__ logmel, const int32_t
     const int nc = f1 - f0;
     const bool active = g < groups;
     const float *src = logmel + (size_t)F0 * n_mels;
+    const float x0 = src[m];
 
     float s = 0.f;
     if (active)
-        for (int f = f0 + g; f < f1; f += groups) s += src[(size_t)f * n_mels + m];
+        for (int f = f0 + g; f < f1; f += groups) s += src[(size_t)f * n_mels + m] - x0;
     if (active) red[g * n_mels + m] = s;
     __syncthreads();
     float mean = 0.f;
@@ -230,7 +235,7 @@ __global__ void mel_stats_kernel(const float *__restrict__ logmel, const int32_t
     float q = 0.f;
     if (active)
         for (int f = f0 + g; f < f1; f += groups) {
-            float d = src[(size_t)f * n_mels + m] - mean;
+            float d = (src[(size_t)f * n_mels + m] - x0) - mean;
             q = fmaf(d, d, q);
         }
     if (active) red[g * n_mels + m] = q;
@@ -273,11 +278,61 @@ __global__ void mel_apply_kernel(const float *__restrict__ logmel, const int32_t
     int f0, f1;
     mel_chunk(c, F, f0, f1);
     const float *src = logmel + (size_t)F0 * n_mels;
+    const float x0 = src[m];
     float *dst = feats + (size_t)F0 * n_mels;
-    for (int f = f0 + g; f < f1; f += groups) dst[(size_t)f * n_mels + m] = (src[(size_t)f * n_mels + m] - mean) * inv;
+    for (int f = f0 + g; f < f1; f += groups) dst[(size_t)f * n_mels + m] = ((src[(size_t)f * n_mels + m] - x0) - mean) * inv;
 }
 
 }  // namespace
+
+MelTables build_mel_tables(int n_mels, const std::function<void *(const void *, size_t)> &upload) {
+    // host, double precision where the reference uses it
+    std::vector<float> win(400);
+    for (int i = 0; i < 400; ++i) win[i] = (float)(0.5 - 0.5 * std::cos(2.0 * M_PI * i / 399.0));  // fft.cpp:1117-1142
+    std::vector<float2> tw256(256), tw512(257);
+    for (int m = 0; m < 256; ++m) tw256[m] = make_float2((float)std::cos(2.0 * M_PI * m / 256.0), (float)-std::sin(2.0 * M_PI * m / 256.0));
+    for (int k = 0; k <= 256; ++k) tw512[k] = make_float2((float)std::cos(2.0 * M_PI * k / 512.0), (float)-std::sin(2.0 * M_PI * k / 512.0));
+    // Slaney filterbank, audio.cpp:18-94
+    auto hz2mel = [](double f) { return f < 1000.0 ? f / (200.0 / 3.0) : 15.0 + std::log(f / 1000.0) / 0.06875177742094912; };
+    auto mel2hz = [](double m) { return m < 15.0 ? m * (200.0 / 3.0) : 1000.0 * std::exp((m - 15.0) * 0.06875177742094912); };
+    const int nm = n_mels, nf = 257;
+    const double mmin = hz2mel(0.0), mmax = hz2mel(8000.0);
+    std::vector<double> hz(nm + 2);
+    for (int i = 0; i < nm + 2; ++i) hz[i] = mel2hz(mmin + (double)i * (mmax - mmin) / (double)(nm + 1));
+    std::vector<float> fbw;
+    std::vector<int32_t> fstart(nm), flen(nm), foff(nm);
+    for (int m = 0; m < nm; ++m) {
+        const double left = hz[m], center = hz[m + 1], right = hz[m + 2], enorm = 2.0 / (right - left);
+        int first = -1, last = -1;
+        std::vector<float> col(nf);
+        for (int f = 0; f < nf; ++f) {
+            const double fr = (double)f * 16000.0 / (2.0 * (nf - 1));
+            double v = 0.0;
+            if (fr >= left && fr <= center && center > left) v = (fr - left) / (center - left);
+            else if (fr > center && fr <= right && right > center) v = (right - fr) / (right - center);
+            col[f] = (float)(v * enorm);
+            if (col[f] != 0.f) {
+                if (first < 0) first = f;
+                last = f;
+            }
+        }
+        fstart[m] = first < 0 ? 0 : first;
+        flen[m] = first < 0 ? 0 : last - first + 1;
+        foff[m] = (int32_t)fbw.size();
+        for (int f = fstart[m]; f < fstart[m] + flen[m]; ++f) fbw.push_back(col[f]);
+    }
+    auto up = [&](const auto &v) { return upload(v.data(), v.size() * sizeof(v[0])); };
+    MelTables tb;
+    tb.window = static_cast<const float *>(up(win));
+    tb.tw256 = static_cast<const float2 *>(up(tw256));
+    tb.tw512 = static_cast<const float2 *>(up(tw512));
+    tb.fb_w = static_cast<const float *>(up(fbw));
+    tb.fb_start = static_cast<const int32_t *>(up(fstart));
+    tb.fb_len = static_cast<const int32_t *>(up(flen));
+    tb.fb_off = static_cast<const int32_t *>(up(foff));
+    tb.fb_nnz = (int)fbw.size();
+    return tb;
+}
 
 size_t mel_smem_bytes(const MelTables &tb) {
     return sizeof(float) * (WIN + 512 + 514 + ((tb.fb_nnz + 3) & ~3) + WARPS * (512 + 512 + 260));
@@ -292,7 +347,7 @@ void launch_mel(const float *pcm, const int64_t *pcm_off, const int32_t *frame_o
     launch_pdl(mel_logpower_kernel<false>, dim3(grid), dim3(WARPS * 32), mel_smem_bytes(tb), st, pcm, pcm_off, frame_off, nullptr, n_mels, tb,
                                                                              normalize ? logmel : feats);
     if (!normalize) return;
-    int groups = 640 / n_mels;  // 8 for 80 bins, 5 for 128
+    int groups = MEL_NORM_THREADS / n_mels;  // 8 for 80 bins, 5 for 128
     launch_pdl(mel_stats_kernel, dim3(MEL_CH, n_utt), dim3(groups * n_mels), sizeof(float) * groups * n_mels, st, logmel, frame_off, n_mels, part);
     launch_pdl(mel_apply_kernel, dim3(MEL_CH, n_utt), dim3(groups * n_mels), 0, st, logmel, frame_off, n_mels, part, feats);
 }

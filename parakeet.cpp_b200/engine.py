@@ -100,7 +100,8 @@ EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_co
            "pk_diar_stream_open", "pk_diar_stream_reset", "pk_diar_stream_step", "pk_diar_stream_step_feats", "pk_diar_stream_speakers",
            "pk_diar_stream_count", "pk_set_boost_rows", "pk_stream_set_boost", "pk_kernel_tdt_decode_boosted",
            "pk_transcribe_diarize_batch", "pk_run_transcribe_diarize_staged", "pk_diarize_transcription", "pk_diarize_words",
-           "pk_lm_load", "pk_lm_free", "pk_lm_order", "pk_lm_count", "pk_lm_sentence_log10", "pk_set_ctc_beam", "pk_kernel_ctc_beam"]
+           "pk_lm_load", "pk_lm_free", "pk_lm_order", "pk_lm_count", "pk_lm_sentence_log10", "pk_set_ctc_beam", "pk_kernel_ctc_beam",
+           "pk_kernel_mel", "pk_kernel_mel_stream", "pk_kernel_subsample_conv1", "pk_kernel_subsample_dw"]
 
 _lib = None
 
@@ -227,6 +228,10 @@ def load_library():
     L.pk_set_ctc_beam.argtypes = [vp, C.c_int32, vp, vp, C.c_float, C.c_float]
     L.pk_kernel_ctc_beam.argtypes = [C.c_int, C.c_int, i32p, C.c_int, C.c_int, f32p, C.c_int, vp, vp, C.c_float, C.c_float, C.c_int,
                                      i32p, i32p, i32p, f32p, i32p, f32p, f32p, i32p, i64p]
+    L.pk_kernel_mel.argtypes = [C.c_int, C.c_int, i64p, f32p, C.c_int, C.c_int, f32p, f32p, i64p]
+    L.pk_kernel_mel_stream.argtypes = [C.c_int, C.c_int, i64p, f32p, i32p, i32p, C.c_int, C.c_int, f32p, i64p]
+    L.pk_kernel_subsample_conv1.argtypes = [C.c_int] * 3 + [i32p, C.c_int, f32p, C.c_int, C.c_int] + [f32p] * 7 + [i64p]
+    L.pk_kernel_subsample_dw.argtypes = [C.c_int] * 3 + [i32p, C.c_int, C.c_int] + [f32p] * 6 + [i64p]
     _lib = L
     return L
 
