@@ -258,15 +258,6 @@ pk_status pk_debug_tdt_passes(pk_engine *e, int64_t *out8);
  * random data (epi_kind: EpiKind of csrc/pk_common.cuh; math: PK_MATH_BF16X3 | PK_MATH_BF16X1). */
 pk_status pk_selftest_gemm(int device, int M, int N, int K, int epi_kind, int math, uint32_t seed,
                            float *max_err, float *max_ref);
-/* GPU self-check of the residual GEMM with the LayerNorm fused into its epilogue (csrc/gemm_tc.cu, N = 512, run in place)
- * against the fp32 GEMM followed by the stand-alone LayerNorm kernel.  mode 0: x = resid + a(A W^T + b), planes = LN1(x);
- * 1: x = LN1(.), planes = LN2(x);  2: x = LN1(.), planes = split(x);  3: mode 0 without a residual.
- * err4 = {max |x - x_ref|, max |x_ref|, max |planes - planes_ref|, max |planes_ref|}. */
-pk_status pk_selftest_gemm_ln(int device, int M, int K, int mode, int math, uint32_t seed, float *err4);
-/* GPU self-check of the wgmma attention kernel (csrc/attention_wgmma.cu: head_dim 64, <= 128 frames per utterance) against the
- * fp32 CUDA-core attention kernel on seeded random inputs (d_model 512, 8 heads), utterance lengths lens[0..n).  mode bit 0:
- * zero position table; bit 1: zero keys.  err2 = {max |ctx - ctx_ref|, max |ctx_ref|}. */
-pk_status pk_selftest_attention(int device, const int32_t *lens, int n, int tmax, int mode, uint32_t seed, float *err2);
 
 /* Kernel test hooks (csrc/kernel_hooks.cu): each runs ONE launcher of the hot path exactly as the engine calls it, on host fp32
  * arrays, on a private stream, synchronously, and returns every output buffer whole (bf16 planes widened to float).  Every
@@ -281,8 +272,8 @@ pk_status pk_selftest_attention(int device, const int32_t *lens, int n, int tmax
 pk_status pk_kernel_gemm(int device, int path, int math, int cluster, int M, int N, int K, int epi_kind, int qcols, int ldo, float alpha,
                          int in_place, const float *A, const float *W, const float *bias, const float *resid, float *out_f32,
                          float *out_hi, float *out_lo, int64_t *guard_bad);
-/* Relative-position attention: kernel 0 = fp32 CUDA-core, 1 = mma.sync (default), 2 = wgmma.  qkv [rows_total][3 d] (kernels 1
- * and 2 get q in fp32 and k | v as bf16 planes, as the EPI_QKV_ACT epilogue lays them out), pp [2 tmax - 1][d], utterance
+/* Relative-position attention: kernel 0 = fp32 CUDA-core, 1 = mma.sync (default).  qkv [rows_total][3 d] (kernel 1 gets q
+ * in fp32 and k | v as bf16 planes, as the EPI_QKV_ACT epilogue lays them out), pp [2 tmax - 1][d], utterance
  * b = rows [row_off[b], row_off[b+1]) (rows outside every utterance may exist).  ctx [rows_total][d]: ctx_f32 with
  * PK_MATH_FP32 (kernel 0 only), else ctx_hi and, with PK_MATH_BF16X3, ctx_lo. */
 pk_status pk_kernel_attention(int device, int kernel, int math, int n_utt, const int32_t *row_off, int rows_total, int d_model, int n_heads,

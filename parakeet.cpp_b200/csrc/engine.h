@@ -162,9 +162,6 @@ struct pk_engine {
     struct GraphEntry { cudaGraphExec_t exec = nullptr; int64_t launches = 0; int seen = 0; };
     std::map<std::string, GraphEntry> graphs;
     bool use_graphs = true;
-    bool attn_wgmma = false;                   // PK_ATTN_UMMA=1 (the switch's name from the earlier design): wgmma attention (attention_wgmma.cu)
-                                               // for head_dim 64 and batches of <= 128-frame utterances.  Off by default: measured on H100 (700 W),
-                                               // 64 x 126 frames, 89 us per launch against 69 us for the mma.sync kernel
     bool attn_tc = true;                       // mma.sync attention for head_dim 64 / 128 (PK_ATTN_TC=0: fp32 kernel)
 
     // ---- the staged batch
@@ -293,15 +290,12 @@ struct pk_engine {
     pk_status set_batch_shapes(const int32_t *n_frames_or_null, const int64_t *offsets_or_null, int n);
     pk_status upload_shapes();
     void gemm(const Act &A, int lda, const GemmWeight &W, int M_, EpiParams epi);
-    // x = resid + alpha * (A . W^T + b) followed by LayerNorm(s): ONE kernel (gemm_tc_ln_kernel) when fuse_ln applies,
-    // else the residual GEMM and layernorm_kernel.  resid_in_x: the residual is x itself (false: x = A . W^T + b).
+    // x = resid + alpha * (A . W^T + b) (the residual GEMM) followed by LayerNorm(s) (layernorm_kernel).  resid_in_x: the
+    // residual is x itself (false: x = A . W^T + b).
     // out_ln1: x receives LayerNorm_1 of the sum (block end) instead of the sum; planes = split of the last LayerNorm.
     pk_status gemm_ln(const Act &A, int lda, const GemmWeight &W, int M_, bool resid_in_x, float alpha, const float *ln1_w, const float *ln1_b,
                       bool out_ln1, const float *ln2_w, const float *ln2_b, ActBuf planes);
     int gemm_cluster = 0;                      // PK_GEMM_CLUSTER=2|4: wide GEMMs (fc1, q/k/v, pw1) run as clusters of 2 | 4 CTAs along N with the A tile multicast
-    bool ln_mcast = false;                     // PK_LN_MCAST=1: the A tile is fetched in quarters and TMA-multicast across the cluster
-    int fuse_ln_min_k = 0;                     // PK_FUSE_LN_MINK: fuse only GEMMs with K >= this
-    bool fuse_ln = false;                      // PK_FUSE_LN=1: LayerNorm in the epilogue of the GEMM that produces its input
     // few-row GEMMs (M <= 128: streaming steps, short utterances) go to gemm_skinny.cu (PK_GEMM_SKINNY=0: never)
     bool skinny = true;
     bool stream_skinny = true;                 // the same for the steps of Sortformer streams (offline diarization keeps skinny off)

@@ -26,9 +26,8 @@
 // 16-B aligned bases and pitches, qcols a multiple of 64): the warpgroup applies epi_math in the fragment layout, writes
 // 64-row x 128-B chunks (SWIZZLE_128B) into its two chunk buffers and stores each with one TMA store of whole rows;
 // RESID_F32 loads its residual chunk by TMA into the same buffer.  Otherwise it writes from registers (epilogue_regs).
-// The cluster forms (gemm_tc_cl_kernel, gemm_tc_ln_kernel) keep the COOPERATIVE body (gemm_tc_body): both consumer
-// warpgroups work on one tile (rows [64 (wg - 1), 64 wg)) and run its epilogue together, which their cluster-wide
-// barriers need.
+// The cluster form (gemm_tc_cl_kernel) keeps the COOPERATIVE body (gemm_tc_body): both consumer warpgroups work on one
+// tile (rows [64 (wg - 1), 64 wg)) and run its epilogue together, which their cluster-wide barriers need.
 // Every spin-wait is bounded and traps, so a protocol bug is an error, not a hung GPU.
 #include <cuda.h>
 
@@ -47,23 +46,20 @@ constexpr int CONSUMER_WARPS = 8;
 // each consumer warpgroup into its own two chunk buffers, and stores them with TMA.
 constexpr int CHUNK_ROWS = 64, CHUNK_BYTES = CHUNK_ROWS * 128;
 
-template <int BN, int NPASS, bool LN = false, bool STAGED = false>
+template <int BN, int NPASS, bool STAGED = false>
 struct TcCfg {
     static constexpr int A_BYTES = BM * BK * 2;                 // one plane, 16 KB
     static constexpr int W_BYTES = BN * BK * 2;
     static constexpr int PLANES = (NPASS == 3) ? 2 : 1;
     static constexpr int STAGE_BYTES = PLANES * (A_BYTES + W_BYTES);
-    static constexpr int STAT_BYTES = LN ? 4 * BM * 4 * 4 : 0;  // fused LayerNorm: 4 exchanges x 128 rows x 4 CTAs (fp32)
     static constexpr int EPI_BYTES = STAGED ? 2 * 2 * CHUNK_BYTES : 0;   // staged epilogue: 2 consumers x 2 chunk buffers
-    static constexpr int AVAIL = 227 * 1024 - STAT_BYTES - EPI_BYTES - 1024 - 256;
+    static constexpr int AVAIL = 227 * 1024 - EPI_BYTES - 1024 - 256;
     static constexpr int STAGES = AVAIL / STAGE_BYTES > 8 ? 8 : AVAIL / STAGE_BYTES;
-    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + STAT_BYTES + EPI_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + EPI_BYTES + 1024 /*align*/ + 256 /*barriers*/;
     static_assert(STAGES >= 2, "pipeline depth");
     static_assert(SMEM <= 227 * 1024, "shared memory per CTA");
     static_assert((2 * STAGES + (STAGED ? 4 : 0)) * 8 <= 256, "barrier space");
 };
-
-constexpr int LN_CL = 4;        // fused LayerNorm: one cluster of 4 CTAs x 128 columns = one 512-wide row block
 
 // Epilogue of one consumer warpgroup: its 64 x BN accumulator slab, rows row0.., columns n0...  Lanes t and t ^ 1 swap
 // the row-(r + 8) pair of one and the row-r pair of the other, so every lane holds 4 consecutive columns of one row --
@@ -362,114 +358,36 @@ __device__ __forceinline__ void epilogue_staged(float (&d)[BN / 2], const EpiPar
     }
 }
 
-// Sum over the cluster of one per-row partial: lane `writer` of each row stores its CTA's partial into slot `rank` of the
-// row in every CTA's buffer, one cluster barrier, then every CTA adds the four slots in the same order.  Every thread of
-// every CTA must call it the same number of times (the barrier).
-__device__ __forceinline__ float cluster_row_sum(float part, float *buf, int lrow, bool writer, uint32_t rank) {
-    if (writer) {
-        const uint32_t a = smem_u32(buf + lrow * LN_CL + rank);
-#pragma unroll
-        for (uint32_t r = 0; r < (uint32_t)LN_CL; ++r) st_cluster_f32(mapa_rank(a, r), part);
-    }
-    cluster_sync();
-    const float4 v = *reinterpret_cast<const float4 *>(buf + lrow * LN_CL);
-    return ((v.x + v.y) + v.z) + v.w;
-}
-
-// Fused LayerNorm epilogue of one consumer warpgroup (BN = 128 columns of a 512-wide row; the row lives in the 4 CTAs of
-// the cluster).  Two passes per LayerNorm like layernorm_kernel: mean, then the centred second moment.
-__device__ __forceinline__ void epilogue_ln(const float (&d)[64], const LnEpi &ep, int row0, int lrow0, int n0, int M, int N, int lane,
-                                            float *stat, uint32_t rank) {
-    const int q = lane & 3;
-    const int row = row0 + (lane >> 2) + ((q & 1) ? 8 : 0), lrow = lrow0 + (lane >> 2) + ((q & 1) ? 8 : 0);
-    const bool writer = (q >> 1) == 0, live = row < M;
-    float x[64];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-        const float s0 = (q & 1) ? d[4 * j] : d[4 * j + 2], s1 = (q & 1) ? d[4 * j + 1] : d[4 * j + 3];
-        const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
-        const float4 v = (q & 1) ? make_float4(r0, r1, d[4 * j + 2], d[4 * j + 3]) : make_float4(d[4 * j], d[4 * j + 1], r0, r1);
-        const int col = n0 + 8 * j + 4 * (q >> 1);
-        float4 b = make_float4(0.f, 0.f, 0.f, 0.f), r = b;
-        if (ep.bias) b = __ldg(reinterpret_cast<const float4 *>(ep.bias + col));
-        if (ep.resid && live) r = *reinterpret_cast<const float4 *>(ep.resid + (size_t)row * N + col);
-        x[4 * j] = r.x + ep.alpha * (v.x + b.x);
-        x[4 * j + 1] = r.y + ep.alpha * (v.y + b.y);
-        x[4 * j + 2] = r.z + ep.alpha * (v.z + b.z);
-        x[4 * j + 3] = r.w + ep.alpha * (v.w + b.w);
-    }
-    auto store_f32 = [&]() {
-        if (!live || !ep.out_f32) return;
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-            *reinterpret_cast<float4 *>(ep.out_f32 + (size_t)row * N + n0 + 8 * j + 4 * (q >> 1)) =
-                make_float4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
-    };
-    auto layernorm = [&](const float *w, const float *bb, float *buf) {
-        float s = 0.f;
-#pragma unroll
-        for (int i = 0; i < 64; ++i) s += x[i];
-        s += __shfl_xor_sync(0xffffffffu, s, 2);
-        const float mean = cluster_row_sum(s, buf, lrow, writer, rank) / (float)N;
-        float c = 0.f;
-#pragma unroll
-        for (int i = 0; i < 64; ++i) c += (x[i] - mean) * (x[i] - mean);
-        c += __shfl_xor_sync(0xffffffffu, c, 2);
-        const float rstd = rsqrtf(cluster_row_sum(c, buf + BM * LN_CL, lrow, writer, rank) / (float)N + ep.eps);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            const int col = n0 + 8 * j + 4 * (q >> 1);
-            const float4 g = __ldg(reinterpret_cast<const float4 *>(w + col)), o = __ldg(reinterpret_cast<const float4 *>(bb + col));
-            x[4 * j] = (x[4 * j] - mean) * rstd * g.x + o.x;
-            x[4 * j + 1] = (x[4 * j + 1] - mean) * rstd * g.y + o.y;
-            x[4 * j + 2] = (x[4 * j + 2] - mean) * rstd * g.z + o.z;
-            x[4 * j + 3] = (x[4 * j + 3] - mean) * rstd * g.w + o.w;
-        }
-    };
-    if (!ep.out_ln1) store_f32();
-    layernorm(ep.ln1_w, ep.ln1_b, stat);
-    if (ep.out_ln1) store_f32();
-    if (ep.ln2_w) layernorm(ep.ln2_w, ep.ln2_b, stat + 2 * BM * LN_CL);
-    if (live) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-            store_act4(ep.planes, (size_t)row * N + n0 + 8 * j + 4 * (q >> 1), make_float4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]));
-    }
-}
-
-// The cooperative kernel body of the cluster forms below.
-// CL > 1: thread-block clusters of CL CTAs along N.  The CL CTAs of a cluster work on the SAME 128-row block and on adjacent
-// column tiles, so the A tile of a k-block is the same for all of them.  MC: each CTA fetches 128 / CL of its rows (tmA_*
-// then have a 128 / CL-row box) and TMA-multicasts the slice into the stage of every CTA of the cluster; a stage is then
-// written by all CTAs, so its "empty" barrier collects the arrivals of the consumer warps of all of them.
-// LN: the fused LayerNorm epilogue (CL = 4, N = 512, one unit per cluster: grid = 4 x row blocks).
-template <int BN, int NPASS, int EK, int CL, bool MC, bool LN>
+// The cooperative kernel body of the cluster form below: thread-block clusters of CL CTAs along N.  The CL CTAs of a cluster
+// work on the SAME 128-row block and on adjacent column tiles, so the A tile of a k-block is the same for all of them.  Each
+// CTA fetches 128 / CL of its rows (tmA_* then have a 128 / CL-row box) and TMA-multicasts the slice into the stage of every
+// CTA of the cluster; a stage is then written by all CTAs, so its "empty" barrier collects the arrivals of the consumer warps
+// of all of them.
+template <int BN, int NPASS, int EK, int CL>
 __device__ __forceinline__ void gemm_tc_body(const CUtensorMap &tmA_hi, const CUtensorMap &tmA_lo, const CUtensorMap &tmW_hi,
-                                             const CUtensorMap &tmW_lo, int M, int N, int K, const EpiParams &epi, const LnEpi &lnp) {
-    using C = TcCfg<BN, NPASS, LN>;
+                                             const CUtensorMap &tmW_lo, int M, int N, int K, const EpiParams &epi) {
+    using C = TcCfg<BN, NPASS>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    float *stat = reinterpret_cast<float *>(tiles + (size_t)C::STAGES * C::STAGE_BYTES);
-    uint64_t *full = reinterpret_cast<uint64_t *>(tiles + (size_t)C::STAGES * C::STAGE_BYTES + C::STAT_BYTES), *empty = full + C::STAGES;
+    uint64_t *full = reinterpret_cast<uint64_t *>(tiles + (size_t)C::STAGES * C::STAGE_BYTES), *empty = full + C::STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
     const int nkb = K / BK;
     const int tiles_n = (N + BN - 1) / BN, tiles_m = (M + BM - 1) / BM;
     // work units: the cluster walks (row block, group of CL column tiles); this CTA takes column tile `rank` of the group
-    // (tiles_n % CL == 0, checked by the launchers)
-    const uint32_t rank = CL > 1 ? cluster_ctarank() : 0u;
+    // (tiles_n % CL == 0, checked by the launcher)
+    const uint32_t rank = cluster_ctarank();
     const int group_n = tiles_n / CL, num_units = group_n * tiles_m;
     const int first = (int)blockIdx.x / CL, step = (int)gridDim.x / CL;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < C::STAGES; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], CONSUMER_WARPS * (MC ? CL : 1));
+            mbar_init(&empty[s], CONSUMER_WARPS * CL);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (CL > 1) cluster_sync();      // every CTA's barriers exist before a peer multicasts into it / arrives on them
-    else __syncthreads();
+    cluster_sync();      // every CTA's barriers exist before a peer multicasts into it / arrives on them
     pdl_wait();      // barriers are set up while the previous grid drains; now its results are visible
     pdl_trigger();
 
@@ -485,26 +403,18 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap &tmA_hi, const CU
                     mbar_wait(&empty[s], ph ^ 1);
                     uint8_t *st = tiles + (size_t)s * C::STAGE_BYTES;
                     mbar_expect_tx(&full[s], C::STAGE_BYTES);
-                    if (MC) {       // this CTA's slice of the A rows, into the stage of every CTA of the cluster
-                        constexpr int SL = BM / CL, SLB = SL * BK * 2;
-                        constexpr uint16_t mask = (uint16_t)((1u << CL) - 1u);
-                        tma_load_2d_mcast(st + rank * SLB, &tmA_hi, &full[s], kb * BK, m0 + (int)rank * SL, mask);
-                        if (NPASS == 3) tma_load_2d_mcast(st + C::A_BYTES + C::W_BYTES + rank * SLB, &tmA_lo, &full[s], kb * BK, m0 + (int)rank * SL, mask);
-                    } else {
-                        tma_load_2d(st, &tmA_hi, &full[s], kb * BK, m0);
-                        if (NPASS == 3) tma_load_2d(st + C::A_BYTES + C::W_BYTES, &tmA_lo, &full[s], kb * BK, m0);
-                    }
+                    // this CTA's slice of the A rows, into the stage of every CTA of the cluster
+                    constexpr int SL = BM / CL, SLB = SL * BK * 2;
+                    constexpr uint16_t mask = (uint16_t)((1u << CL) - 1u);
+                    tma_load_2d_mcast(st + rank * SLB, &tmA_hi, &full[s], kb * BK, m0 + (int)rank * SL, mask);
+                    if (NPASS == 3) tma_load_2d_mcast(st + C::A_BYTES + C::W_BYTES + rank * SLB, &tmA_lo, &full[s], kb * BK, m0 + (int)rank * SL, mask);
                     tma_load_2d(st + C::A_BYTES, &tmW_hi, &full[s], kb * BK, n0);
                     if (NPASS == 3) tma_load_2d(st + 2 * C::A_BYTES + C::W_BYTES, &tmW_lo, &full[s], kb * BK, n0);
                 }
             }
             pdl_trigger_late();     // every operand load of this CTA has been issued
         }
-        __syncwarp();                // the elected lane rejoins its warp before the .aligned cluster barriers below
-        if (LN) {                    // the producer warpgroup takes part in the epilogue's cluster barriers
-            const int n_sync = lnp.ln2_w ? 4 : 2;
-            for (int i = 0; i < n_sync; ++i) cluster_sync();
-        }
+        __syncwarp();                // the elected lane rejoins its warp before the .aligned cluster barrier at the end
     } else {
         // ===================== consumers: wgmma + epilogue =====================
         const int cw = wg - 1;                              // row half of the tile
@@ -512,13 +422,9 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap &tmA_hi, const CU
         auto release = [&](int s) {                         // this warp has finished reading stage s
             __syncwarp();
             if (lane == 0) {
-                if (MC) {
-                    const uint32_t a = smem_u32(&empty[s]);
+                const uint32_t a = smem_u32(&empty[s]);
 #pragma unroll
-                    for (uint32_t r = 0; r < (uint32_t)CL; ++r) mbar_arrive_cluster(mapa_rank(a, r));
-                } else {
-                    mbar_arrive(&empty[s]);
-                }
+                for (uint32_t r = 0; r < (uint32_t)CL; ++r) mbar_arrive_cluster(mapa_rank(a, r));
             }
         };
         uint32_t it = 0;
@@ -556,11 +462,10 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap &tmA_hi, const CU
             fence_operands(d);
             if (prev_s >= 0) release(prev_s);
             const int lrow0 = cw * 64 + (warp & 3) * 16;
-            if constexpr (LN) epilogue_ln(d, lnp, m0 + lrow0, lrow0, n0, M, N, lane, stat, rank);
-            else epilogue_regs<BN, EK>(d, epi, m0 + lrow0, n0, M, N, lane);
+            epilogue_regs<BN, EK>(d, epi, m0 + lrow0, n0, M, N, lane);
         }
     }
-    if (CL > 1) cluster_sync();      // nobody leaves while a peer may still multicast into it / arrive on its barriers
+    cluster_sync();      // nobody leaves while a peer may still multicast into it / arrive on its barriers
 }
 
 // The default GEMM, in the ping-pong form: each consumer warpgroup owns whole 128 x BN tiles (the CTA's units alternate
@@ -576,7 +481,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, int M, int N,
                int K, const __grid_constant__ EpiParams epi, const __grid_constant__ EpiMaps om) {
-    using C = TcCfg<BN, NPASS, false, STAGED>;
+    using C = TcCfg<BN, NPASS, STAGED>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t *chunks = tiles + (size_t)C::STAGES * C::STAGE_BYTES;
@@ -708,16 +613,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(TC_THREADS, 1)
 gemm_tc_cl_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                   const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, int M, int N,
                   int K, const __grid_constant__ EpiParams epi) {
-    gemm_tc_body<128, NPASS, EK, CL, true, false>(tmA_hi, tmA_lo, tmW_hi, tmW_lo, M, N, K, epi, LnEpi());
-}
-
-// residual GEMM + fused LayerNorm(s): clusters of 4 CTAs = one 512-column row block; MC = A tile multicast
-template <int NPASS, bool MC>
-__global__ void __cluster_dims__(LN_CL, 1, 1) __launch_bounds__(TC_THREADS, 1)
-gemm_tc_ln_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-                  const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, int M, int N,
-                  int K, const __grid_constant__ LnEpi lnp) {
-    gemm_tc_body<128, NPASS, EPI_BIAS_F32, LN_CL, MC, true>(tmA_hi, tmA_lo, tmW_hi, tmW_lo, M, N, K, EpiParams(), lnp);
+    gemm_tc_body<128, NPASS, EK, CL>(tmA_hi, tmA_lo, tmW_hi, tmW_lo, M, N, K, epi);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
@@ -785,7 +681,7 @@ bool staged_maps(EpiMaps *om, const EpiParams &e, int M, int N) {
 
 template <int BN, int NPASS, int EK, bool STAGED>
 cudaError_t launch_k(const TcOperand &A, const TcOperand &W, int M, int N, int K, const EpiParams &epi, const EpiMaps &om, cudaStream_t st) {
-    using C = TcCfg<BN, NPASS, false, STAGED>;
+    using C = TcCfg<BN, NPASS, STAGED>;
     static PerDeviceFlag attr_flag;
     bool &attr = attr_flag.cur();
     if (!attr) {
@@ -855,20 +751,6 @@ cudaError_t launch_kcl(const TcOperand &A_sl, const TcOperand &W, int M, int N, 
     return launch_pdl(gemm_tc_cl_kernel<NPASS, EK, CL>, dim3((unsigned)(ncl * CL)), dim3(TC_THREADS), C::SMEM, st, A_sl.hi, alo, W.hi, wlo, M, N, K, epi);
 }
 
-template <int NPASS, bool MC>
-cudaError_t launch_ln(const TcOperand &A, const TcOperand &W, int M, int N, int K, const LnEpi &ep, cudaStream_t st) {
-    using C = TcCfg<128, NPASS, true>;
-    static PerDeviceFlag attr_flag;
-    if (!attr_flag.cur()) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_tc_ln_kernel<NPASS, MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
-        if (e != cudaSuccess) return e;
-        attr_flag.cur() = true;
-    }
-    const CUtensorMap &alo = (NPASS == 3) ? A.lo : A.hi, &wlo = (NPASS == 3) ? W.lo : W.hi;
-    const int row_blocks = (M + BM - 1) / BM;
-    return launch_pdl(gemm_tc_ln_kernel<NPASS, MC>, dim3((unsigned)(LN_CL * row_blocks)), dim3(TC_THREADS), C::SMEM, st, A.hi, alo, W.hi, wlo, M, N, K, ep);
-}
-
 }  // namespace
 
 bool make_tc_operand(TcOperand *out, const bf16 *hi, const bf16 *lo, uint64_t rows, uint64_t K, uint32_t box_rows) {
@@ -903,7 +785,7 @@ cudaError_t launch_gemm_tc(const TcOperand &A, const TcOperand &W, int M, int N,
     if (K % BK != 0 || A.box_rows != BM) return cudaErrorInvalidValue;
     if (split3 && !(A.has_lo && W.has_lo)) return cudaErrorInvalidValue;
     if (cl > 1 && split3 && A_slice && A_slice->has_lo && (int)A_slice->box_rows * cl == BM && W.box_rows == 128 && gemm_tc_cluster_supported(N, epi.kind, cl)) {
-        // clusters of `cl` CTAs along N, A tile multicast (gemm_tc_body, CL > 1)
+        // clusters of `cl` CTAs along N, A tile multicast (gemm_tc_body)
         switch (epi.kind) {
         case EPI_BIAS_SILU_ACT: return cl == 2 ? launch_kcl<3, EPI_BIAS_SILU_ACT, 2>(*A_slice, W, M, N, K, epi, st) : launch_kcl<3, EPI_BIAS_SILU_ACT, 4>(*A_slice, W, M, N, K, epi, st);
         case EPI_GLU_F32: return cl == 2 ? launch_kcl<3, EPI_GLU_F32, 2>(*A_slice, W, M, N, K, epi, st) : launch_kcl<3, EPI_GLU_F32, 4>(*A_slice, W, M, N, K, epi, st);
@@ -912,17 +794,6 @@ cudaError_t launch_gemm_tc(const TcOperand &A, const TcOperand &W, int M, int N,
     }
     if (W.box_rows == 128) return split3 ? launch_t<128, 3>(A, W, M, N, K, epi, st) : launch_t<128, 1>(A, W, M, N, K, epi, st);
     if (W.box_rows == 64) return split3 ? launch_t<64, 3>(A, W, M, N, K, epi, st) : launch_t<64, 1>(A, W, M, N, K, epi, st);
-    return cudaErrorInvalidValue;
-}
-
-bool gemm_tc_ln_supported(int N) { return N == LN_CL * 128; }
-
-cudaError_t launch_gemm_tc_ln(const TcOperand &A, const TcOperand &W, int M, int N, int K, bool split3, const LnEpi &epi, cudaStream_t st) {
-    if (M <= 0) return cudaSuccess;
-    if (!gemm_tc_ln_supported(N) || K % BK != 0 || W.box_rows != 128 || !epi.ln1_w || !epi.ln1_b) return cudaErrorInvalidValue;
-    if (split3 && !(A.has_lo && W.has_lo)) return cudaErrorInvalidValue;
-    if (A.box_rows == BM / LN_CL) return split3 ? launch_ln<3, true>(A, W, M, N, K, epi, st) : launch_ln<1, true>(A, W, M, N, K, epi, st);
-    if (A.box_rows == BM) return split3 ? launch_ln<3, false>(A, W, M, N, K, epi, st) : launch_ln<1, false>(A, W, M, N, K, epi, st);
     return cudaErrorInvalidValue;
 }
 

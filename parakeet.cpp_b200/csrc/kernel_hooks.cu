@@ -199,12 +199,11 @@ pk_status pk_kernel_gemm(int device, int path, int math, int cluster, int M, int
 pk_status pk_kernel_attention(int device, int kernel, int math, int n_utt, const int32_t *row_off, int rows_total, int d_model, int n_heads,
                               int tmax, const float *qkv, const float *pp, const float *pos_u, const float *pos_v, float *ctx_f32,
                               float *ctx_hi, float *ctx_lo, int64_t *guard_bad) {
-    if (kernel < 0 || kernel > 2 || !offsets_ok(row_off, n_utt, rows_total) || n_heads < 1 || d_model % n_heads || tmax < 1 || !qkv || !pp ||
+    if (kernel < 0 || kernel > 1 || !offsets_ok(row_off, n_utt, rows_total) || n_heads < 1 || d_model % n_heads || tmax < 1 || !qkv || !pp ||
         !pos_u || !pos_v)
         return PK_ERR_INVALID;
     const int hd = d_model / n_heads, maxT = max_len(row_off, n_utt);
     if (maxT > tmax || maxT < 1) return PK_ERR_INVALID;
-    if (kernel == 2 && !relpos_attention_wgmma_supported(hd, maxT)) return PK_ERR_INVALID;
     // the output is what the engine's ctx buffer holds in that math mode: fp32, or bf16 hi (| lo) planes
     const bool f32 = math == PK_MATH_FP32;
     if (f32 ? (kernel != 0 || !ctx_f32) : (!ctx_hi || (math == PK_MATH_BF16X3) != (ctx_lo != nullptr))) return PK_ERR_INVALID;
@@ -238,9 +237,7 @@ pk_status pk_kernel_attention(int device, int kernel, int math, int n_utt, const
         ActBuf spp; spp.hi = pph; spp.lo = ppl;
         launch_split(dkv, hkv.size(), skv, cx.st);
         launch_split(dpp, (size_t)NP * d, spp, cx.st);
-        launched = kernel == 1
-                       ? launch_relpos_attention_tc(dq32, du, dv, kvh, kvl, 2 * d, doff, n_utt, maxT, n_heads, hd, pph, ppl, tmax, d, out, cx.st)
-                       : launch_relpos_attention_wgmma(dq32, du, dv, kvh, kvl, 2 * d, doff, n_utt, maxT, n_heads, hd, pph, ppl, tmax, d, out, cx.st);
+        launched = launch_relpos_attention_tc(dq32, du, dv, kvh, kvl, 2 * d, doff, n_utt, maxT, n_heads, hd, pph, ppl, tmax, d, out, cx.st);
     }
     if (!launched) return PK_ERR_INVALID;
     pk_status rc = cx.finish(guard_bad);

@@ -108,24 +108,6 @@ bool gemm_tc_cluster_supported(int N, int epi_kind, int cl);
 cudaError_t launch_gemm_tc(const TcOperand &A, const TcOperand &W, int M, int N, int K, bool split3,
                            const EpiParams &epi, cudaStream_t st, int cl = 1, const TcOperand *A_slice = nullptr);
 
-// Residual GEMM + fused LayerNorm (gemm_tc.cu, the same wgmma main loop):
-//     v = resid + alpha * (A . W^T + bias)   (resid may be null);   y1 = LN1(v);   y2 = LN2(y1) if ln2_w
-//     out_f32 = out_ln1 ? y1 : v   (may alias resid);   planes = hi/lo split of the last LayerNorm's result
-// N must be a full LayerNorm row of 4 x 128 columns (one 4-CTA cluster per 128-row block; row statistics through
-// distributed shared memory).  A with a 32-row box (A.box_rows == 32): every CTA fetches a quarter of the A tile and
-// TMA-multicasts it to the cluster; with the 128-row box every CTA loads the whole tile.
-struct LnEpi {
-    const float *bias = nullptr, *resid = nullptr;
-    float alpha = 1.0f;
-    float *out_f32 = nullptr;
-    const float *ln1_w = nullptr, *ln1_b = nullptr, *ln2_w = nullptr, *ln2_b = nullptr;
-    bool out_ln1 = false;
-    ActBuf planes;
-    float eps = 1e-5f;
-};
-bool gemm_tc_ln_supported(int N);
-cudaError_t launch_gemm_tc_ln(const TcOperand &A, const TcOperand &W, int M, int N, int K, bool split3, const LnEpi &epi, cudaStream_t st);
-
 // ------------------------------------------------------------------ gemm_skinny.cu (M <= 128: the streaming path's GEMMs)
 size_t gemm_skinny_ws_floats(int max_n, int max_splits);
 cudaError_t launch_gemm_skinny(const bf16 *Ahi, const bf16 *Alo, int lda, const bf16 *Whi, const bf16 *Wlo, int M, int N, int K, bool split3,
@@ -151,13 +133,6 @@ bool launch_relpos_attention(const float *qkv, int ld_qkv, const int32_t *row_of
 bool launch_relpos_attention_tc(const float *q32, const float *pos_u, const float *pos_v, const bf16 *kv_hi, const bf16 *kv_lo,
                                 int ld_kv, const int32_t *row_off, int n_utt, int max_T, int n_heads, int head_dim, const bf16 *pp_hi,
                                 const bf16 *pp_lo, int tmax, int d_model, ActBuf out, cudaStream_t st);
-
-// wgmma variant (attention_wgmma.cu): head_dim 64, utterances of <= 128 frames, one CTA per (head, utterance); same
-// operands as launch_relpos_attention_tc.
-bool relpos_attention_wgmma_supported(int head_dim, int max_T);
-bool launch_relpos_attention_wgmma(const float *q32, const float *pos_u, const float *pos_v, const bf16 *kv_hi, const bf16 *kv_lo, int ld_kv,
-                                   const int32_t *row_off, int n_utt, int max_T, int n_heads, int head_dim, const bf16 *pp_hi, const bf16 *pp_lo,
-                                   int tmax, int d_model, ActBuf out, cudaStream_t st);
 
 // ------------------------------------------------------------------ attention_mha.cu / speaker_head.cu (Sortformer)
 // Plain multi-head attention (transformer.cpp:15-50) over packed utterances, head_dim 24 only (false otherwise): qkv fp32

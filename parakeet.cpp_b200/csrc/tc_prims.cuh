@@ -91,9 +91,6 @@ __device__ __forceinline__ uint32_t mapa_rank(uint32_t saddr, uint32_t rank) {
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
     asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
-__device__ __forceinline__ void st_cluster_f32(uint32_t cluster_addr, float v) {
-    asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(cluster_addr), "f"(v) : "memory");
-}
 
 // One elected lane of a fully active warp: ptxas then knows that exactly one thread runs the region.
 __device__ __forceinline__ bool elect_one() {

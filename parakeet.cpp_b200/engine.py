@@ -86,7 +86,7 @@ EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_co
            "pk_mel_frames", "pk_encoder_frames", "pk_mel", "pk_encode", "pk_decode", "pk_ctc_logprobs",
            "pk_transcribe_batch", "pk_stage_pcm", "pk_prefetch_pcm", "pk_run_staged", "pk_fetch_tokens", "pk_sync",
            "pk_token_buffer", "pk_stream", "pk_launch_count", "pk_profile_begin", "pk_profile_end",
-           "pk_profile_names", "pk_flush_l2", "pk_selftest_gemm", "pk_selftest_gemm_ln", "pk_selftest_attention",
+           "pk_profile_names", "pk_flush_l2", "pk_selftest_gemm",
            "pk_kernel_gemm", "pk_kernel_attention", "pk_kernel_layernorm", "pk_kernel_dwconv", "pk_kernel_ctc_argmax", "pk_kernel_tdt_decode", "pk_kernel_stream_attention", "pk_kernel_stream_dwconv",
            "pk_debug_tdt_phases", "pk_vocab_load", "pk_vocab_free", "pk_vocab_size",
            "pk_detokenize", "pk_group_words", "pk_tokenize", "pk_ctc_decode_boosted",
@@ -158,8 +158,6 @@ def load_library():
     L.pk_debug_tdt_phases.argtypes = [vp, i64p]
     L.pk_debug_tdt_passes.argtypes = [vp, i64p]
     L.pk_selftest_gemm.argtypes = [C.c_int] * 6 + [C.c_uint32, f32p, f32p]
-    L.pk_selftest_gemm_ln.argtypes = [C.c_int] * 5 + [C.c_uint32, f32p]
-    L.pk_selftest_attention.argtypes = [C.c_int, i32p, C.c_int, C.c_int, C.c_int, C.c_uint32, f32p]
     L.pk_kernel_gemm.argtypes = [C.c_int] * 10 + [C.c_float, C.c_int] + [f32p] * 7 + [i64p]
     L.pk_kernel_attention.argtypes = [C.c_int] * 4 + [i32p] + [C.c_int] * 4 + [f32p] * 7 + [i64p]
     L.pk_kernel_layernorm.argtypes = [C.c_int] * 3 + [f32p] * 5 + [C.c_int] * 2 + [f32p] * 4 + [i64p]
@@ -517,27 +515,6 @@ def selftest_gemm(M, N, K, epi_kind, math=0, seed=1, device=0):
     if st != 0:
         raise RuntimeError(f"pk_selftest_gemm failed ({st})")
     return e.value, r.value
-
-
-def selftest_attention(lens, tmax=126, mode=0, seed=1, device=0):
-    """-> (max_abs_err, max_abs_ref) of the wgmma attention kernel vs the fp32 attention kernel."""
-    L = load_library()
-    ln = np.ascontiguousarray(lens, np.int32)
-    out = np.zeros(2, np.float32)
-    st = L.pk_selftest_attention(device, _i32p(ln), len(ln), tmax, mode, seed, _f32p(out))
-    if st != 0:
-        raise RuntimeError(f"pk_selftest_attention failed ({st})")
-    return float(out[0]), float(out[1])
-
-
-def selftest_gemm_ln(M, K, mode, math=0, seed=1, device=0):
-    """-> (x_err, x_ref, planes_err, planes_ref) of the fused residual-GEMM + LayerNorm kernel vs fp32 GEMM + LayerNorm kernel."""
-    L = load_library()
-    out = np.zeros(4, np.float32)
-    st = L.pk_selftest_gemm_ln(device, M, K, mode, math, seed, _f32p(out))
-    if st != 0:
-        raise RuntimeError(f"pk_selftest_gemm_ln failed ({st})")
-    return tuple(float(v) for v in out)
 
 
 def _f32p(a):

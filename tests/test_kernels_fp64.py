@@ -386,23 +386,17 @@ ATTN_CFGS = {  # (d, heads): T values
     (512, 8): [1, 2, 15, 16, 17, 63, 64, 65, 127, 128, 129, 192, 193, 376],
     (1024, 8): [1, 63, 64, 65, 113, 128, 129, 376],
 }
-ATTN_KERNELS = [(0, MATH_F32), (1, MATH_X3), (1, MATH_X1), (2, MATH_X3)]
-
-
-def _kernel_ok(kernel, d, H, maxT):
-    return kernel != 2 or (d // H == 64 and maxT <= 128)
+ATTN_KERNELS = [(0, MATH_F32), (1, MATH_X3), (1, MATH_X1)]
 
 
 @gpu
-@pytest.mark.parametrize("kernel,math_mode", ATTN_KERNELS, ids=["fp32", "mma-x3", "mma-x1", "wgmma-x3"])
+@pytest.mark.parametrize("kernel,math_mode", ATTN_KERNELS, ids=["fp32", "mma-x3", "mma-x1"])
 @pytest.mark.parametrize("cfg", list(ATTN_CFGS), ids=lambda c: f"d{c[0]}h{c[1]}")
 def test_attention_against_fp64(pkg, kernel, math_mode, cfg):
     """Ragged batches of every length (tmax = the longest, and larger), then each length alone at a non-zero row offset
     inside NaN sentinel rows, then the score regimes on a ragged batch."""
     d, H = cfg
-    lens = [t for t in ATTN_CFGS[cfg] if _kernel_ok(kernel, d, H, t)]
-    if not lens:
-        pytest.skip("no length this kernel supports")
+    lens = ATTN_CFGS[cfg]
     worst = 0.0
     for seed in SEEDS:
         rng = np.random.default_rng(seed * 101 + d + kernel)
@@ -433,7 +427,7 @@ def test_attention_against_fp64(pkg, kernel, math_mode, cfg):
 
 
 @gpu
-@pytest.mark.parametrize("kernel,math_mode", [(0, MATH_F32), (1, MATH_X3), (2, MATH_X3)], ids=["fp32", "mma-x3", "wgmma-x3"])
+@pytest.mark.parametrize("kernel,math_mode", [(0, MATH_F32), (1, MATH_X3)], ids=["fp32", "mma-x3"])
 def test_attention_bound_rejects_mutations(pkg, kernel, math_mode):
     d, H = 512, 8
     lens = [65, 17, 128, 40]
@@ -451,6 +445,19 @@ def test_attention_bound_rejects_mutations(pkg, kernel, math_mode):
         r = check_attention(tuple(None if a is None else a[rows] for a in out), off[:n + 1], int(off[n]), mref[rows], bd[rows])
         report(f"attention kernel {kernel} mutation {name}", r)
         assert r > 1.0, name
+
+
+def test_attention_hook_rejects_unknown_kernel(pkg):
+    """kernel is 0 (fp32) or 1 (mma.sync); any other value is refused with PK_ERR_INVALID before the device is touched."""
+    L = pkg.load_library()
+    d, H, tmax = 512, 8, 4
+    ro = np.array([0, tmax], np.int32)
+    qkv, pp, u, v = np.zeros((tmax, 3 * d), np.float32), np.zeros((2 * tmax - 1, d), np.float32), np.zeros(d, np.float32), np.zeros(d, np.float32)
+    oh, ol = np.zeros((tmax, d), np.float32), np.zeros((tmax, d), np.float32)
+    for kernel in (2, -1):
+        st = L.pk_kernel_attention(0, kernel, MATH_X3, 1, i32p(ro), tmax, d, H, tmax, f32p(qkv), f32p(pp), f32p(u), f32p(v),
+                                   f32p(None), f32p(oh), f32p(ol), C.byref(C.c_int64(-1)))
+        assert st == 1, (kernel, st)
 
 
 # ----------------------------------------------------------------------------------------------------------- LayerNorm
