@@ -32,6 +32,7 @@
 #include <fstream>
 #include <functional>
 #include <iterator>
+#include <limits>
 #include <memory>
 #include <stdexcept>
 #include <string>
@@ -86,6 +87,18 @@ struct TranscribeResult {
     std::vector<int> token_ids;
     std::vector<TimestampedToken> timestamped_tokens;
     std::vector<WordTimestamp> word_timestamps;
+};
+// Transcriber::align (not in the reference): CTC forced alignment of a known text (pk_set_align_targets; DESIGN.md section
+// 15).  text = the detokenised ids that were aligned (Tokenizer::encode skips bytes no piece covers); aligned = false when
+// the audio has too few frames for the tokens (then there are no timestamps and both scores are -inf); log_prob = the
+// best path's score, ctc_log_likelihood = log p(tokens | audio).
+struct AlignResult {
+    std::string text;
+    std::vector<int> token_ids;
+    std::vector<TimestampedToken> timestamped_tokens;
+    std::vector<WordTimestamp> word_timestamps;
+    bool aligned = false;
+    double log_prob = 0.0, ctc_log_likelihood = 0.0;
 };
 // CTC_BEAM (not in the reference): CTC prefix beam search of beam_width hypotheses, fused with the language model of
 // Transcriber::set_language_model when one is set (pk_set_ctc_beam).  It does not combine with boost_phrases.
@@ -328,6 +341,7 @@ class EngineHolder {
     }
     const pk_config &cfg() const { return cfg_; }
     pk_engine *raw() { return e_; }
+    int32_t cap() const { return cap_; }
 
   private:
     pk_config cfg_;
@@ -500,6 +514,61 @@ class Transcriber : public detail::TranscriberBase<Transcriber> {
     void clear_language_model() {
         lm_.reset();
         beam_dirty_ = true;
+    }
+    // CTC forced alignment of `text` in the audio (AlignResult above); a WAV at any rate is converted on the device.
+    AlignResult align(const std::string &audio_path, const std::string &text) {
+        int sr = 16000;
+        auto s = read_audio_native(audio_path, sr);
+        return align(s.data(), s.size(), text, sr);
+    }
+    AlignResult align(const std::vector<float> &samples, const std::string &text) { return align(samples.data(), samples.size(), text); }
+    AlignResult align(const float *samples, size_t n, const std::string &text, int sample_rate = 16000) {
+        return align_chunk({samples}, {n}, {text}, sample_rate)[0];
+    }
+    // Many utterances, max_batch at a time, each with its own text.
+    std::vector<AlignResult> align_batch(const std::vector<std::vector<float>> &utts, const std::vector<std::string> &texts) {
+        if (utts.size() != texts.size()) throw std::invalid_argument("align_batch: one text per utterance expected");
+        std::vector<AlignResult> out;
+        const size_t B = (size_t)eng_->cfg().max_batch;
+        for (size_t i = 0; i < utts.size(); i += B) {
+            std::vector<const float *> p;
+            std::vector<size_t> n;
+            std::vector<std::string> t;
+            for (size_t k = i; k < utts.size() && k < i + B; ++k) { p.push_back(utts[k].data()); n.push_back(utts[k].size()); t.push_back(texts[k]); }
+            for (auto &r : align_chunk(p, n, t, 16000)) out.push_back(std::move(r));
+        }
+        return out;
+    }
+
+  private:
+    std::vector<AlignResult> align_chunk(const std::vector<const float *> &pcm, const std::vector<size_t> &n, const std::vector<std::string> &texts,
+                                         int sample_rate) {
+        std::vector<std::vector<int>> ids;
+        std::vector<int32_t> flat, off{0};
+        for (const auto &t : texts) {
+            ids.push_back(tokenizer_.encode(t));
+            flat.insert(flat.end(), ids.back().begin(), ids.back().end());
+            off.push_back((int32_t)flat.size());
+        }
+        const int32_t none = 0;
+        if (pk_set_align_targets(eng_->raw(), flat.empty() ? &none : flat.data(), off.data(), (int32_t)texts.size()) != PK_OK)
+            throw std::runtime_error(std::string("parakeet_b200: ") + pk_last_error(eng_->raw()));
+        auto rows = eng_->run(pcm, n, PK_DECODER_CTC_ALIGN, sample_rate);
+        std::vector<double> sc(rows.size()), ll(rows.size());
+        if (pk_fetch_align_scores(eng_->raw(), sc.data(), ll.data()) != PK_OK)
+            throw std::runtime_error(std::string("parakeet_b200: ") + pk_last_error(eng_->raw()));
+        std::vector<AlignResult> out(rows.size());
+        for (size_t b = 0; b < rows.size(); ++b) {
+            AlignResult &r = out[b];
+            r.token_ids = ids[b];
+            r.text = tokenizer_.decode(ids[b]);
+            r.timestamped_tokens = rows[b];
+            r.word_timestamps = tokenizer_.group(rows[b]);
+            r.log_prob = sc[b];
+            r.ctc_log_likelihood = ll[b];
+            r.aligned = sc[b] != -std::numeric_limits<double>::infinity();
+        }
+        return out;
     }
 };
 

@@ -39,8 +39,9 @@ typedef enum {
 
 /* PK_DECODER_TDT runs only on a TDT model, PK_DECODER_RNNT only on an RNN-T model (n_durations = 0);
  * PK_DECODER_CTC needs a CTC head (has_ctc).  A mismatch is PK_ERR_INVALID.  PK_DECODER_CTC_BEAM: CTC prefix beam
- * search with optional word n-gram fusion (pk_set_ctc_beam below; DESIGN.md section 14). */
-typedef enum { PK_DECODER_CTC = 0, PK_DECODER_TDT = 1, PK_DECODER_RNNT = 2, PK_DECODER_CTC_BEAM = 3 } pk_decoder;
+ * search with optional word n-gram fusion (pk_set_ctc_beam below; DESIGN.md section 14).  PK_DECODER_CTC_ALIGN: CTC forced
+ * alignment of known token sequences (pk_set_align_targets below; DESIGN.md section 15). */
+typedef enum { PK_DECODER_CTC = 0, PK_DECODER_TDT = 1, PK_DECODER_RNNT = 2, PK_DECODER_CTC_BEAM = 3, PK_DECODER_CTC_ALIGN = 4 } pk_decoder;
 
 /* GEMM arithmetic.  PK_MATH_BF16X3 (default): wgmma MMAs on bf16
  * hi/lo operand splits, 3 MMAs per product (hi*hi + hi*lo + lo*hi), fp32
@@ -494,6 +495,43 @@ pk_status pk_kernel_ctc_beam(int device, int n_utt, const int32_t *row_off, int 
                              const pk_lm *lm, const pk_vocab *vocab, float alpha, float beta, int cap, int32_t *tok, int32_t *t_start,
                              int32_t *t_end, float *t_conf, int32_t *topk_id, float *topk_lp, float *blank_lp, int32_t *bp,
                              int64_t *guard_bad);
+
+/* ---- CTC forced alignment (DESIGN.md section 15 defines it): the timestamps of a KNOWN token sequence y_1..y_L per
+ * utterance, by the Viterbi pass over the CTC trellis of z = (blank, y_1, blank, ..., y_L, blank) (blank = vocab - 1),
+ * S = 2L + 1 states, on the fp32 log-probs lp[t][v] of the CTC head, accumulated in double:
+ *   delta_0(0) = lp[0][blank], delta_0(1) = lp[0][y_1], other states -inf;
+ *   delta_t(s) = lp[t][z_s] + max(delta_{t-1}(s), delta_{t-1}(s-1), delta_{t-1}(s-2)), the s-2 term only when z_s is not
+ *   blank and z_s != z_{s-2}; ties prefer s, then s-1, then s-2.  The path ends in S-1 or S-2, whichever is larger (a tie
+ *   goes to S-1); the alignment score is that maximum.  The CTC log-likelihood log p(y | x) is the same trellis with
+ *   log-sum-exp in place of max, lse(alpha_{T-1}(S-1), alpha_{T-1}(S-2)).
+ * A row with T < L + R frames (R = number of i with y_i = y_{i+1}), or whose best path has probability 0, cannot be aligned:
+ * it gets zero tokens and both scores are -inf (a per-row outcome, not an error).  L = 0 aligns every frame to blank.
+ * The path's label of every frame goes through the greedy CTC collapse, so a row of pk_tokens has the layout and meaning of
+ * a greedy CTC row: start = first frame of the token, end = the frame before the next token's (the last token ends at
+ * T-1), conf = exp(lp[start][token]).  Aligning the greedy transcript gives back the greedy row.
+ *   pk_set_align_targets  : the token ids of each row of the next PK_DECODER_CTC_ALIGN run, row i = ids[offsets[i] ..
+ *                           offsets[i+1]), n_rows <= max_batch (n_rows = 0 clears them; ids and offsets may then be NULL).  The
+ *                           ids are copied (ordered on the engine stream, no synchronisation) into buffers that never move,
+ *                           so one CUDA graph per batch shape serves every set of targets.  PK_ERR_INVALID: an id outside
+ *                           0..vocab-2 (the blank included; pk_last_error names the row), decreasing offsets, a model without
+ *                           a CTC head, a Sortformer engine.  PK_ERR_CAPACITY: a row of more than PK_ALIGN_MAX_TOKENS ids.
+ *                           Either error leaves the previous targets in force.
+ *   pk_fetch_align_scores : the alignment score and log p(y | x) of each row of the last run (either pointer may be NULL);
+ *                           PK_ERR_INVALID when the last run was not an alignment.
+ * PK_DECODER_CTC_ALIGN works through pk_run_staged, pk_transcribe_batch, pk_decode and jobs; it is PK_ERR_INVALID without
+ * targets, with a number of target rows other than the batch's, on a model without a CTC head, on a Sortformer engine, and
+ * in pk_transcribe_diarize_batch / pk_run_transcribe_diarize_staged.  Phrase boosting does not change an alignment. */
+#define PK_ALIGN_MAX_TOKENS 2048
+pk_status pk_set_align_targets(pk_engine *e, const int32_t *ids, const int32_t *offsets, int32_t n_rows);
+pk_status pk_fetch_align_scores(pk_engine *e, double *score, double *loglik);
+/* Kernel test hook (conventions of the pk_kernel_* hooks): the alignment kernel and the greedy collapse as the engine
+ * launches them, on host log-probs [rows][V] (blank = V - 1), utterance b = rows [row_off[b], row_off[b+1]), with targets
+ * b = tgt[tgt_off[b] .. tgt_off[b+1]).  Outputs, all guarded: tok [n_utt][1 + cap] (len, ids), t_start / t_end / t_conf
+ * [n_utt][cap], score / loglik [n_utt], path [rows] (the best path's state of every frame, -1 in an infeasible row).  Any
+ * output but tok may be NULL.  Errors as pk_set_align_targets. */
+pk_status pk_kernel_ctc_align(int device, int n_utt, const int32_t *row_off, int rows, int V, const float *logprobs, const int32_t *tgt,
+                              const int32_t *tgt_off, int cap, int32_t *tok, int32_t *t_start, int32_t *t_end, float *t_conf, double *score,
+                              double *loglik, int32_t *path, int64_t *guard_bad);
 
 /* Offline speaker diarization: Sortformer (include/parakeet/sortformer.hpp, src/sortformer.cpp:42-122 of the reference).
  * PCM -> log-mel WITHOUT per-bin normalisation (main.cpp:514-517) -> NEST encoder (the offline FastConformer under keys

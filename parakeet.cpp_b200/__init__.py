@@ -15,4 +15,4 @@ from .engine import (Decoder, Engine, ModelConfig, TranscribeOptions, Transcribe
                      make_rnnt_600m_config, make_tiny_rnnt_config, make_nemotron_600m_config,
                      make_tiny_nemotron_config, SortformerConfig, DiarizationSegment, diar_segments,
                      make_sortformer_117m_config, make_tiny_sortformer_config, AOSCCache, DiarizedWord,
-                     DiarizedResult, DiarizedTranscriber, diarize_transcription, diarize_words, LanguageModel)
+                     DiarizedResult, DiarizedTranscriber, diarize_transcription, diarize_words, LanguageModel, AlignResult)

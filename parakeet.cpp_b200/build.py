@@ -22,7 +22,7 @@ LIB = os.path.join(HERE, "libparakeet_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-diag-suppress", "550"]
-CU = ["mel.cu", "subsample.cu", "gemm_simt.cu", "gemm_tc.cu", "gemm_skinny.cu", "attention.cu", "attention_tc.cu", "attention_mha.cu", "speaker_head.cu", "norm_conv.cu", "ctc.cu", "ctc_beam.cu",
+CU = ["mel.cu", "subsample.cu", "gemm_simt.cu", "gemm_tc.cu", "gemm_skinny.cu", "attention.cu", "attention_tc.cu", "attention_mha.cu", "speaker_head.cu", "norm_conv.cu", "ctc.cu", "ctc_beam.cu", "ctc_align.cu",
       "tdt.cu", "stream.cu", "stream_engine.cu", "resample.cu", "engine.cu",
       "kernel_hooks.cu"]
 CPP = ["safetensors.cpp", "text.cpp", "nccl_dl.cpp", "lm.cpp"]

@@ -757,6 +757,31 @@ pk_status pk_engine::run_ctc_beam() {
     return PK_OK;
 }
 
+// PK_DECODER_CTC_ALIGN: the CTC head and frame pass as run_ctc_beam (log-probs into the idle qkv workspace), then the
+// alignment of the targets of pk_set_align_targets, one CTA per utterance (ctc_align.cu), which overwrites the frame
+// labels and confidences of the arg-max with its best path, then the greedy collapse of that path.
+pk_status pk_engine::run_ctc_align() {
+    const pk_config &c = cfg;
+    if ((size_t)M * c.vocab > (size_t)Bmax * Tmax * 3 * c.d_model) return fail(PK_ERR_CAPACITY, "CTC alignment: workspace too small for the log-probs");
+    const int ldv = (c.vocab + 3) & ~3;
+    EpiParams ep;
+    ep.kind = EPI_BIAS_F32;
+    ep.out_f32 = logits;
+    ep.ldo = ldv;
+    gemm(enc_operand(this), c.d_model, ctc_head, M, ep);
+    {
+        Scope sc(this, CAT_CTC);
+        launch_ctc_frame_argmax(logits, M, c.vocab, ldv, best, bconf, qkv, stream);
+        launch_ctc_align(qkv, d_row_off, n_utt, c.vocab, align_ids, align_off, align_bp, align_stride, best, bconf, align_score,
+                         align_loglik, nullptr, stream);
+        launch_ctc_collapse(best, bconf, d_row_off, n_utt, c.vocab - 1, cap, tok, t_start, t_end, t_conf, stream);
+    }
+    launches += 3;
+    last_tdt = false;
+    PK_CUDA(cudaGetLastError());
+    return PK_OK;
+}
+
 pk_status pk_engine::run_tdt() {
     const pk_config &c = cfg;
     // enc_proj for all frames at once (joint's first Linear, tdt.cpp:17)
@@ -1450,12 +1475,23 @@ static pk_status check_decoder(pk_engine *e, pk_decoder dec) {
         if (e->boosting()) return e->fail(PK_ERR_INVALID, "PK_DECODER_CTC_BEAM: phrase boosting is set (beam search does not boost)");
         return PK_OK;
     }
+    if (dec == PK_DECODER_CTC_ALIGN) {
+        if (!e->cfg.has_ctc) return e->fail(PK_ERR_INVALID, "PK_DECODER_CTC_ALIGN: this model has no CTC head");
+        if (!e->align_rows) return e->fail(PK_ERR_INVALID, "PK_DECODER_CTC_ALIGN: call pk_set_align_targets first");
+        return PK_OK;
+    }
     const bool rnnt_model = e->cfg.n_durations == 0;
     if (dec == PK_DECODER_TDT && rnnt_model)
         return e->fail(PK_ERR_INVALID, "PK_DECODER_TDT on an RNN-T model (n_durations = 0): use PK_DECODER_RNNT");
     if (dec == PK_DECODER_RNNT && !rnnt_model)
         return e->fail(PK_ERR_INVALID, "PK_DECODER_RNNT on a TDT model: use PK_DECODER_TDT");
     return PK_OK;
+}
+// The targets must name every row of the staged batch (checked once the batch is staged)
+static pk_status check_align_rows(pk_engine *e, pk_decoder dec) {
+    if (dec != PK_DECODER_CTC_ALIGN || e->align_rows == e->n_utt) return PK_OK;
+    return e->fail(PK_ERR_INVALID, "PK_DECODER_CTC_ALIGN: the targets have " + std::to_string(e->align_rows) + " rows, the batch " +
+                                       std::to_string(e->n_utt));
 }
 static pk_status run_pipeline(pk_engine *e, pk_decoder dec) {   // everything after the front end
     pk_status s;
@@ -1471,6 +1507,7 @@ pk_status pk_run_staged(pk_engine *e, pk_decoder dec) {
     cudaSetDevice(e->device);
     if (e->gemm_err) return e->gemm_err;
     if (pk_status ds = check_decoder(e, dec)) return ds;
+    if (pk_status ds = check_align_rows(e, dec)) return ds;
     {
         pk_status fs = run_front(e);
         e->front_done = false;      // a second pk_run_staged of the same staged batch re-runs the front end
@@ -1480,7 +1517,9 @@ pk_status pk_run_staged(pk_engine *e, pk_decoder dec) {
 }
 
 static pk_status run_asr_graph(pk_engine *e, pk_decoder dec) {
-    std::string key(1, dec == PK_DECODER_CTC ? 'c' : (dec == PK_DECODER_RNNT ? 'r' : (dec == PK_DECODER_CTC_BEAM ? 'B' : 't')));
+    e->align_last = false;
+    // (the alignment targets live in buffers that never move: one 'a' graph serves every set of targets)
+    std::string key(1, dec == PK_DECODER_CTC ? 'c' : (dec == PK_DECODER_RNNT ? 'r' : (dec == PK_DECODER_CTC_BEAM ? 'B' : (dec == PK_DECODER_CTC_ALIGN ? 'a' : 't'))));
     if (dec == PK_DECODER_CTC_BEAM) {                   // width, tables, weights: pk_set_ctc_beam drops the 'B' graphs of old tables
         const int32_t wg[2] = {e->beam_w, e->beam_gen};
         const double ab[2] = {e->beam_lm.alpha_ln10, e->beam_lm.beta};
@@ -1491,7 +1530,9 @@ static pk_status run_asr_graph(pk_engine *e, pk_decoder dec) {
     const int32_t bg = e->brows_on ? -1 : (e->boost_on ? e->boost_gen : 0);
     key.append(reinterpret_cast<const char *>(&bg), sizeof(bg));
     key.append(reinterpret_cast<const char *>(e->frame_off.data()), e->frame_off.size() * sizeof(int32_t));
-    return e->run_graphed(key, [e, dec]() { return run_pipeline(e, dec); });
+    const pk_status s = e->run_graphed(key, [e, dec]() { return run_pipeline(e, dec); });
+    e->align_last = s == PK_OK && dec == PK_DECODER_CTC_ALIGN;
+    return s;
 }
 
 pk_status pk_fetch_tokens(pk_engine *e, pk_tokens *out) {
@@ -1862,6 +1903,67 @@ pk_status pk_set_ctc_beam(pk_engine *e, int32_t width, const pk_lm *lm, const pk
     return PK_OK;
 }
 
+pk_status pk_set_align_targets(pk_engine *e, const int32_t *ids, const int32_t *offsets, int32_t n_rows) {
+    if (!e || n_rows < 0 || (n_rows > 0 && !offsets)) return PK_ERR_INVALID;
+    if (e->diar) return e->fail(PK_ERR_INVALID, "pk_set_align_targets: a Sortformer engine has no decoder");
+    if (!e->cfg.has_ctc) return e->fail(PK_ERR_INVALID, "pk_set_align_targets: this model has no CTC head");
+    if (n_rows > e->Bmax) return e->fail(PK_ERR_CAPACITY, "pk_set_align_targets: more rows than pk_config.max_batch");
+    for (int32_t i = 0; i < n_rows; ++i) {
+        if (offsets[i] < 0 || offsets[i + 1] < offsets[i]) return e->fail(PK_ERR_INVALID, "pk_set_align_targets: offsets must be non-decreasing");
+        if (offsets[i + 1] - offsets[i] > PK_ALIGN_MAX_TOKENS)
+            return e->fail(PK_ERR_CAPACITY, "pk_set_align_targets: row " + std::to_string(i) + " has " + std::to_string(offsets[i + 1] - offsets[i]) +
+                                                " tokens; a row holds at most " + std::to_string(PK_ALIGN_MAX_TOKENS));
+    }
+    const int32_t n_ids = n_rows > 0 ? offsets[n_rows] - offsets[0] : 0;
+    if (n_ids > 0 && !ids) return PK_ERR_INVALID;
+    for (int32_t i = 0; i < n_rows; ++i)
+        for (int32_t k = offsets[i]; k < offsets[i + 1]; ++k)
+            if (ids[k] < 0 || ids[k] > e->cfg.vocab - 2)
+                return e->fail(PK_ERR_INVALID, "pk_set_align_targets: row " + std::to_string(i) + " has token id " + std::to_string(ids[k]) +
+                                                   " (ids are 0.." + std::to_string(e->cfg.vocab - 2) + "; the blank is not a target)");
+    cudaSetDevice(e->device);
+    if (n_rows == 0) {
+        e->align_rows = 0;
+        return PK_OK;
+    }
+    if (!e->align_ids) {
+        e->align_stride = 2 * std::min(e->Tmax, PK_ALIGN_MAX_TOKENS) + 1;
+        e->align_ids = e->dalloc<int32_t>((size_t)e->Bmax * PK_ALIGN_MAX_TOKENS);
+        e->align_off = e->dalloc<int32_t>((size_t)e->Bmax + 1);
+        e->align_bp = e->dalloc<uint8_t>((size_t)e->Bmax * e->Tmax * e->align_stride);
+        e->align_score = e->dalloc<double>(e->Bmax);
+        e->align_loglik = e->dalloc<double>(e->Bmax);
+        if (!e->align_ids || !e->align_off || !e->align_bp || !e->align_score || !e->align_loglik) {
+            e->align_ids = nullptr;
+            return e->fail(PK_ERR_CUDA, "cudaMalloc failed (alignment workspace)");
+        }
+    }
+    // Host copies (pageable): cudaMemcpyAsync has read them when it returns, and the copies are ordered after the runs
+    // still queued on the stream that read the previous targets.
+    std::vector<int32_t> hid(ids ? ids + offsets[0] : nullptr, ids ? ids + offsets[0] + n_ids : nullptr), hoff(n_rows + 1);
+    for (int32_t i = 0; i <= n_rows; ++i) hoff[i] = offsets[i] - offsets[0];
+    cudaError_t ce = n_ids > 0 ? cudaMemcpyAsync(e->align_ids, hid.data(), (size_t)n_ids * sizeof(int32_t), cudaMemcpyHostToDevice, e->stream)
+                               : cudaSuccess;
+    if (ce == cudaSuccess) ce = cudaMemcpyAsync(e->align_off, hoff.data(), hoff.size() * sizeof(int32_t), cudaMemcpyHostToDevice, e->stream);
+    if (ce != cudaSuccess) return e->fail(PK_ERR_CUDA, std::string("pk_set_align_targets: ") + cudaGetErrorString(ce));
+    e->align_rows = n_rows;
+    return PK_OK;
+}
+
+pk_status pk_fetch_align_scores(pk_engine *e, double *score, double *loglik) {
+    if (!e) return PK_ERR_INVALID;
+    if (e->diar) return e->fail(PK_ERR_INVALID, "pk_fetch_align_scores: a Sortformer engine has no decoder");
+    if (!e->align_last) return e->fail(PK_ERR_INVALID, "pk_fetch_align_scores: the last run was not an alignment (PK_DECODER_CTC_ALIGN)");
+    cudaSetDevice(e->device);
+    cudaError_t ce = score ? cudaMemcpyAsync(score, e->align_score, (size_t)e->n_utt * sizeof(double), cudaMemcpyDeviceToHost, e->stream)
+                           : cudaSuccess;
+    if (ce == cudaSuccess && loglik)
+        ce = cudaMemcpyAsync(loglik, e->align_loglik, (size_t)e->n_utt * sizeof(double), cudaMemcpyDeviceToHost, e->stream);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
+    if (ce != cudaSuccess) return e->fail(PK_ERR_CUDA, std::string("pk_fetch_align_scores: ") + cudaGetErrorString(ce));
+    return PK_OK;
+}
+
 pk_status pk_set_boost(pk_engine *e, const int32_t *phrase_ids, const int32_t *phrase_off, int32_t n_phrases, float boost) {
     if (!e || n_phrases < 0 || (n_phrases > 0 && (!phrase_ids || !phrase_off))) return PK_ERR_INVALID;
     if (e->diar) return e->fail(PK_ERR_INVALID, "pk_set_boost: a Sortformer engine has no decoder");
@@ -2015,8 +2117,11 @@ pk_status pk_decode(pk_engine *e, const float *enc, const int32_t *enc_lens, int
     cudaSetDevice(e->device);
     pk_status s;
     if ((s = check_decoder(e, dec))) return s;
+    e->align_last = false;
     if ((s = stage_enc(e, enc, enc_lens, n_utt))) return s;
+    if ((s = check_align_rows(e, dec))) return s;
     if ((s = e->run_decoder(dec))) return s;
+    e->align_last = dec == PK_DECODER_CTC_ALIGN;
     return e->fetch(out);
 }
 
@@ -2027,6 +2132,7 @@ pk_status pk_ctc_logprobs(pk_engine *e, const float *enc, int32_t total_frames, 
     if (total_frames > e->Tmax) return e->fail(PK_ERR_CAPACITY, "pk_ctc_logprobs: more than Tmax frames");
     pk_status s;
     int32_t len = total_frames;
+    e->align_last = false;
     if ((s = stage_enc(e, enc, &len, 1))) return s;
     // the [M][V] log-prob matrix lands in the (idle) qkv workspace
     if ((size_t)e->M * e->cfg.vocab > (size_t)e->Bmax * e->Tmax * 3 * e->cfg.d_model)

@@ -222,6 +222,14 @@ struct pk_engine {
     int32_t *beam_topk_id = nullptr, *beam_bp = nullptr;
     float *beam_topk_lp = nullptr, *beam_blank = nullptr;
 
+    // ---- CTC forced alignment (pk_set_align_targets), buffers allocated by its first call and never moved
+    int align_rows = 0;                                // rows of the targets in place (0: none)
+    int32_t *align_ids = nullptr, *align_off = nullptr;   // [Bmax][PK_ALIGN_MAX_TOKENS] packed ids, [Bmax + 1] offsets
+    uint8_t *align_bp = nullptr;                       // [Bmax Tmax][align_stride] back-pointers
+    int align_stride = 0;                              // 2 min(Tmax, PK_ALIGN_MAX_TOKENS) + 1
+    double *align_score = nullptr, *align_loglik = nullptr;   // [Bmax] each
+    bool align_last = false;                           // the token buffer holds an alignment (pk_fetch_align_scores)
+
     // ---- optional per-kernel-class timing (CUDA events on the engine stream)
     enum { CAT_MEL, CAT_SUBSAMPLE, CAT_GEMM, CAT_LAYERNORM, CAT_ATTENTION, CAT_DWCONV, CAT_CTC, CAT_TDT, CAT_MHA, CAT_HEAD, CAT_N };
     struct ProfRec { int cat; cudaEvent_t a, b; double flops; };
@@ -316,7 +324,9 @@ struct pk_engine {
     pk_status run_ctc(float *logprobs_dev_or_null);
     pk_status run_tdt();
     pk_status run_ctc_beam();
+    pk_status run_ctc_align();
     pk_status run_decoder(pk_decoder dec) {           // (dec already checked)
+        if (dec == PK_DECODER_CTC_ALIGN) return run_ctc_align();
         return dec == PK_DECODER_CTC ? run_ctc(nullptr) : (dec == PK_DECODER_CTC_BEAM ? run_ctc_beam() : run_tdt());
     }
     pk_status fetch(pk_tokens *out);

@@ -746,6 +746,49 @@ extern "C" pk_status pk_kernel_ctc_beam(int device, int n_utt, const int32_t *ro
     return PK_OK;
 }
 
+extern "C" pk_status pk_kernel_ctc_align(int device, int n_utt, const int32_t *row_off, int rows, int V, const float *logprobs,
+                                         const int32_t *tgt, const int32_t *tgt_off, int cap, int32_t *tok, int32_t *t_start,
+                                         int32_t *t_end, float *t_conf, double *score, double *loglik, int32_t *path,
+                                         int64_t *guard_bad) {
+    if (V < 2 || rows < 0 || cap < 1 || !tok || (rows > 0 && !logprobs) || !offsets_ok(row_off, n_utt, rows) || !tgt_off ||
+        tgt_off[0] != 0)
+        return PK_ERR_INVALID;
+    for (int b = 0; b < n_utt; ++b) {
+        if (tgt_off[b + 1] < tgt_off[b]) return PK_ERR_INVALID;
+        if (tgt_off[b + 1] - tgt_off[b] > PK_ALIGN_MAX_TOKENS) return PK_ERR_CAPACITY;
+    }
+    const int n_tgt = tgt_off[n_utt];
+    if (n_tgt > 0 && !tgt) return PK_ERR_INVALID;
+    for (int i = 0; i < n_tgt; ++i)
+        if (tgt[i] < 0 || tgt[i] > V - 2) return PK_ERR_INVALID;
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const size_t R = std::max(rows, 1);
+    const int stride = 2 * std::min(max_len(row_off, n_utt), PK_ALIGN_MAX_TOKENS) + 1;   // as the engine sizes it from Tmax
+    const float *dlp = cx.upload(logprobs, (size_t)rows * V);
+    const int32_t *doff = cx.upload(row_off, (size_t)n_utt + 1);
+    const int32_t *dtg = cx.upload(tgt, (size_t)n_tgt), *dto = cx.upload(tgt_off, (size_t)n_utt + 1);
+    uint8_t *dbp = static_cast<uint8_t *>(cx.alloc(R * stride));
+    int32_t *dbest = static_cast<int32_t *>(cx.alloc(R * sizeof(int32_t)));
+    float *dconf = static_cast<float *>(cx.alloc(R * sizeof(float)));
+    int32_t *dtok = cx.guarded<int32_t>((size_t)n_utt * (1 + cap));
+    int32_t *dst = cx.guarded<int32_t>((size_t)n_utt * cap), *den = cx.guarded<int32_t>((size_t)n_utt * cap);
+    float *dcf = cx.guarded<float>((size_t)n_utt * cap);
+    double *dsc = cx.guarded<double>(n_utt), *dll = cx.guarded<double>(n_utt);
+    int32_t *dpath = cx.guarded<int32_t>(R);
+    if (!cx.ok) return PK_ERR_CUDA;
+    launch_ctc_align(dlp, doff, n_utt, V, dtg, dto, dbp, stride, dbest, dconf, dsc, dll, dpath, cx.st);
+    launch_ctc_collapse(dbest, dconf, doff, n_utt, V - 1, cap, dtok, dst, den, dcf, cx.st);
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    auto get = [](void *h, const void *d, size_t bytes) { return !h || cudaMemcpy(h, d, bytes, cudaMemcpyDeviceToHost) == cudaSuccess; };
+    if (!get(tok, dtok, (size_t)n_utt * (1 + cap) * 4) || !get(t_start, dst, (size_t)n_utt * cap * 4) ||
+        !get(t_end, den, (size_t)n_utt * cap * 4) || !get(t_conf, dcf, (size_t)n_utt * cap * 4) || !get(score, dsc, (size_t)n_utt * 8) ||
+        !get(loglik, dll, (size_t)n_utt * 8) || !get(path, dpath, (size_t)rows * 4))
+        return PK_ERR_CUDA;
+    return PK_OK;
+}
+
 namespace {
 
 int conv_len3(int n) { return (n - 1) / 2 + 1; }   // 3 taps, stride 2, padding 1

@@ -253,6 +253,20 @@ void launch_ctc_beam(const float *logprobs, const int32_t *topk_id, const float 
                      const int32_t *row_off, int n_utt, int V, int width, int cap, const DeviceLM &lm, const DevicePieces &pieces,
                      int32_t *bp, int32_t *tok, int32_t *t_start, int32_t *t_end, float *t_conf, cudaStream_t st);
 
+// ------------------------------------------------------------------ ctc_align.cu (CTC forced alignment, DESIGN.md section 15)
+constexpr int CTC_ALIGN_THREADS = 256;
+// Dynamic shared memory of the alignment kernel: double-buffered Viterbi and forward rows of 2 PK_ALIGN_MAX_TOKENS + 1
+// states, and the targets.
+size_t ctc_align_smem_bytes();
+// One CTA per utterance b: the targets tgt[tgt_off[b] .. tgt_off[b+1]) (ids in 0..V-2, at most PK_ALIGN_MAX_TOKENS) aligned
+// to the log-probs of rows [row_off[b], row_off[b+1]).  Back-pointers bp [rows][bp_stride] (bp_stride >= 2 L + 1 of every
+// feasible row); the best path's label and exp(log-prob) of every frame into best / conf (blank everywhere in an
+// infeasible row), the Viterbi score and the log-likelihood into score / loglik [n_utt] (-inf: infeasible), and, when path
+// is not NULL, the path's state of every frame (-1: infeasible).
+void launch_ctc_align(const float *logprobs, const int32_t *row_off, int n_utt, int V, const int32_t *tgt, const int32_t *tgt_off,
+                      uint8_t *bp, int bp_stride, int32_t *best, float *conf, double *score, double *loglik, int32_t *path,
+                      cudaStream_t st);
+
 // ------------------------------------------------------------------ tdt.cu (K10)
 struct TdtParams {
     int P, J, V, D, L, Bpad, n_utt, cap, max_steps, n_dur;

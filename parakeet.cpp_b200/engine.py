@@ -101,7 +101,8 @@ EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_co
            "pk_diar_stream_count", "pk_set_boost_rows", "pk_stream_set_boost", "pk_kernel_tdt_decode_boosted",
            "pk_transcribe_diarize_batch", "pk_run_transcribe_diarize_staged", "pk_diarize_transcription", "pk_diarize_words",
            "pk_lm_load", "pk_lm_free", "pk_lm_order", "pk_lm_count", "pk_lm_sentence_log10", "pk_set_ctc_beam", "pk_kernel_ctc_beam",
-           "pk_kernel_mel", "pk_kernel_mel_stream", "pk_kernel_subsample_conv1", "pk_kernel_subsample_dw"]
+           "pk_kernel_mel", "pk_kernel_mel_stream", "pk_kernel_subsample_conv1", "pk_kernel_subsample_dw",
+           "pk_set_align_targets", "pk_fetch_align_scores", "pk_kernel_ctc_align"]
 
 _lib = None
 
@@ -226,6 +227,11 @@ def load_library():
     L.pk_set_ctc_beam.argtypes = [vp, C.c_int32, vp, vp, C.c_float, C.c_float]
     L.pk_kernel_ctc_beam.argtypes = [C.c_int, C.c_int, i32p, C.c_int, C.c_int, f32p, C.c_int, vp, vp, C.c_float, C.c_float, C.c_int,
                                      i32p, i32p, i32p, f32p, i32p, f32p, f32p, i32p, i64p]
+    f64p = C.POINTER(C.c_double)
+    L.pk_set_align_targets.argtypes = [vp, i32p, i32p, C.c_int32]
+    L.pk_fetch_align_scores.argtypes = [vp, f64p, f64p]
+    L.pk_kernel_ctc_align.argtypes = [C.c_int, C.c_int, i32p, C.c_int, C.c_int, f32p, i32p, i32p, C.c_int, i32p, i32p, i32p, f32p,
+                                      f64p, f64p, i32p, i64p]
     L.pk_kernel_mel.argtypes = [C.c_int, C.c_int, i64p, f32p, C.c_int, C.c_int, f32p, f32p, i64p]
     L.pk_kernel_mel_stream.argtypes = [C.c_int, C.c_int, i64p, f32p, i32p, i32p, C.c_int, C.c_int, f32p, i64p]
     L.pk_kernel_subsample_conv1.argtypes = [C.c_int] * 3 + [i32p, C.c_int, f32p, C.c_int, C.c_int] + [f32p] * 7 + [i64p]
@@ -463,6 +469,7 @@ class Decoder(enum.IntEnum):          # transcribe.hpp:34
     TDT = 1
     RNNT = 2
     CTC_BEAM = 3                      # CTC prefix beam search (Engine.set_ctc_beam; DESIGN.md section 14)
+    CTC_ALIGN = 4                     # CTC forced alignment of known tokens (Engine.set_align_targets; DESIGN.md section 15)
 
 
 @dataclass
@@ -487,6 +494,19 @@ class TranscribeResult:               # transcribe.hpp:23-30
     token_ids: List[int] = field(default_factory=list)
     timestamped_tokens: List[TimestampedToken] = field(default_factory=list)
     word_timestamps: List[WordTimestamp] = field(default_factory=list)
+
+
+@dataclass
+class AlignResult:
+    """Transcriber.align: the tokens of the text (what was aligned, detokenised), their frames, the words, whether the
+    audio could be aligned at all, the alignment (best path) score and the CTC log-likelihood log p(tokens | audio)."""
+    text: str = ""
+    token_ids: List[int] = field(default_factory=list)
+    timestamped_tokens: List[TimestampedToken] = field(default_factory=list)
+    word_timestamps: List[WordTimestamp] = field(default_factory=list)
+    aligned: bool = False
+    log_prob: float = float("-inf")
+    ctc_log_likelihood: float = float("-inf")
 
 
 @dataclass
@@ -863,6 +883,20 @@ class Engine:
                                            float(alpha), float(beta)), "pk_set_ctc_beam")
 
     # -- non-16 kHz input: converted on the device (SURVEY.md section 8f row 4)
+    def set_align_targets(self, token_lists: Sequence[Sequence[int]]):
+        """The token ids to align in each row of the next Decoder.CTC_ALIGN run (pk_set_align_targets); [] clears them."""
+        flat = np.array([t for ids in token_lists for t in ids] or [0], np.int32)
+        off = np.zeros(len(token_lists) + 1, np.int32)
+        off[1:] = np.cumsum([len(ids) for ids in token_lists])
+        self._check(self.L.pk_set_align_targets(self.h, _i32p(flat), _i32p(off), len(token_lists)), "pk_set_align_targets")
+
+    def align_scores(self, n: int):
+        """(alignment score, log p(tokens | audio)) of each of the n rows of the last alignment run; -inf: not alignable."""
+        sc, ll = np.zeros(max(n, 1), np.float64), np.zeros(max(n, 1), np.float64)
+        self._check(self.L.pk_fetch_align_scores(self.h, sc.ctypes.data_as(C.POINTER(C.c_double)),
+                                                 ll.ctypes.data_as(C.POINTER(C.c_double))), "pk_fetch_align_scores")
+        return [(float(sc[i]), float(ll[i])) for i in range(n)]
+
     def stage_rate(self, pcms: Sequence[np.ndarray], src_rate: int):
         buf, off = _pack(pcms)
         self._check(self.L.pk_stage_pcm_rate(self.h, _f32p(buf), _i64p(off), len(pcms), src_rate), "pk_stage_pcm_rate")
@@ -1113,6 +1147,30 @@ class Transcriber:
         samples = read_wav(audio) if isinstance(audio, str) else np.asarray(audio, np.float32)
         toks = self.engine.transcribe_batch([samples], self._decoder(opts.decoder))[0]
         return self._result(toks, opts.timestamps)
+
+    def align(self, audio, text: str) -> AlignResult:
+        """CTC forced alignment (DESIGN.md section 15): the frames of each token of `text` (tokenised by Tokenizer.encode,
+        which skips bytes no piece covers) and its words in `audio` (a 16 kHz WAV path or samples)."""
+        return self.align_batch([audio], [text])[0]
+
+    def align_batch(self, audios, texts: Sequence[str]) -> List[AlignResult]:
+        if not self.config.has_ctc:
+            raise ValueError("alignment needs a CTC head; this model has none")
+        if len(audios) != len(texts):
+            raise ValueError("align_batch: one text per utterance")
+        pcms = [read_wav(a) if isinstance(a, str) else np.asarray(a, np.float32) for a in audios]
+        targets = [self.tokenizer.encode(t) for t in texts]
+        out = []
+        B = self.config.max_batch
+        for i in range(0, len(pcms), B):
+            self.engine.set_align_targets(targets[i:i + B])
+            rows = self.engine.transcribe_batch(pcms[i:i + B], Decoder.CTC_ALIGN)
+            for ids, toks, (sc, ll) in zip(targets[i:i + B], rows, self.engine.align_scores(len(rows))):
+                r = AlignResult(text=self.tokenizer.decode(ids), token_ids=list(ids), timestamped_tokens=toks,
+                                aligned=sc != float("-inf"), log_prob=sc, ctc_log_likelihood=ll)
+                r.word_timestamps = self.tokenizer.group_words(toks)
+                out.append(r)
+        return out
 
     def transcribe_batch(self, audios, decoder=Decoder.TDT, timestamps: bool = False,
                          options: Optional[Sequence[TranscribeOptions]] = None) -> List[TranscribeResult]:
