@@ -239,25 +239,30 @@ def ref_conv1_dw1(xu, w1, b1, wd, bd, ctx=None, conv1_pad=False):
     return y.transpose(1, 2, 0).reshape(-1, Cn), bd_.transpose(1, 2, 0).reshape(-1, Cn)
 
 
-def ref_dw(xu, wd_tap, bd, prev_row=None, next_row=None):
+def ref_dw(xu, wd_tap, bd, prev_row=None, next_row=None, e_in=None):
     """float64 depthwise 3x3 s2 p1 of one utterance xu [tin][fin][C] -> (y [(t', f')][C], bound).  Mutation: prev_row /
-    next_row [fin][C] = the neighbouring utterances' rows read instead of zeros at t = -1 / tin."""
+    next_row [fin][C] = the neighbouring utterances' rows read instead of zeros at t = -1 / tin.  e_in [tin][fin][C]: a
+    bound on the input's error (a chain of kernels), which adds sum |wd| e_in."""
     tin, fin, Cn = xu.shape
     tout, fout = cl(tin), cl(fin)
     X = np.zeros((tin + 2, fin + 2, Cn))
     X[1:tin + 1, 1:fin + 1] = xu
+    E = np.zeros((tin + 2, fin + 2, Cn))
+    if e_in is not None:
+        E[1:tin + 1, 1:fin + 1] = e_in
     if prev_row is not None:
         X[0, 1:fin + 1] = prev_row
     if next_row is not None:
         X[tin + 1, 1:fin + 1] = next_row
     acc = np.broadcast_to(bd.astype(np.float64), (tout, fout, Cn)).copy()
-    A = np.abs(acc)
+    A, P = np.abs(acc), np.zeros_like(acc)
     for i in range(3):
         for j in range(3):
             t = wd_tap[3 * i + j].astype(np.float64) * X[i:i + 2 * tout:2, j:j + 2 * fout:2]
             acc += t
             A += np.abs(t)
-    return acc.reshape(-1, Cn), (C_SUB * 10 * U * A).reshape(-1, Cn)
+            P += np.abs(wd_tap[3 * i + j].astype(np.float64)) * E[i:i + 2 * tout:2, j:j + 2 * fout:2]
+    return acc.reshape(-1, Cn), (C_SUB * 10 * U * A + P).reshape(-1, Cn)
 
 
 # ----------------------------------------------------------------------------------------------------------- hook runners

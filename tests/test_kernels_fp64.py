@@ -107,18 +107,22 @@ def sig64(x):
 
 
 # ----------------------------------------------------------------------------------------------------------- references
-def ref_gemm(A, W, bias, resid, kind, alpha, math_mode, qcols=0, Ahi_only=False):
-    """float64 linear + epilogue -> (value [M, N'], bound [M, N']), for the q part and the rest when kind is QKV."""
+def ref_gemm(A, W, bias, resid, kind, alpha, math_mode, qcols=0, Ahi_only=False, e_in=None):
+    """float64 linear + epilogue -> (value [M, N'], bound [M, N']), for the q part and the rest when kind is QKV.
+    e_in: a per-element bound on the error of A (a chain of kernels): it adds e_in . |W|^T, and the kernel's own term is
+    taken on |A| + e_in."""
     A64, W64 = A.astype(np.float64), W.astype(np.float64)
     if Ahi_only:                             # mutation: operands rounded to bf16 (hi only)
         A64, W64 = bf16_rn(A).astype(np.float64), bf16_rn(W).astype(np.float64)
     acc = A64 @ W64.T
-    P = np.abs(A64) @ np.abs(W64).T
+    P = (np.abs(A64) if e_in is None else np.abs(A64) + e_in) @ np.abs(W64).T
     K = A.shape[1]
     eps = {MATH_X3: C_X3 * 2.0 ** -16, MATH_X1: C_X1 * 2.0 ** -8, MATH_F32: C_F32 * K * U}[math_mode] * P
     b = np.zeros(W.shape[0]) if bias is None else bias.astype(np.float64)
     v = acc + b
     e = eps + 4 * U * (np.abs(acc) + np.abs(b))
+    if e_in is not None:
+        e = e + e_in @ np.abs(W64).T
     if kind in (EPI["RELU_F32"], EPI["RELU_ACT"]):
         return np.maximum(v, 0), e
     if kind == EPI["SILU_ACT"]:
@@ -287,7 +291,8 @@ def test_gemm_bound_rejects_bf16_hi_only_operands(pkg, path):
 
 
 # ----------------------------------------------------------------------------------------------------------- attention
-def ref_attention(qkv, pp, u, v, row_off, n_utt, d, H, tmax, math_mode, kernel, shift=0, drop_u=False, extra_key=False):
+def ref_attention(qkv, pp, u, v, row_off, n_utt, d, H, tmax, math_mode, kernel, shift=0, drop_u=False, extra_key=False,
+                  e_qkv=None, e_pp=None):
     """float64 relative-position attention per utterance and head:
         S[i,j] = ((q_i + u).k_j + (q_i + v).PP[i - j + tmax - 1]) / sqrt(hd) over keys j < T of the same utterance,
         ctx_i = softmax(S[i]) V.
@@ -295,7 +300,10 @@ def ref_attention(qkv, pp, u, v, row_off, n_utt, d, H, tmax, math_mode, kernel, 
     = D_i (eps_s = 3 * 2^-16 per bf16x3 product on the tensor cores, hd u for the fp32 dot products); a score error D_i
     moves each softmax weight by at most a factor (1 +- 2 D_i), so ctx moves by <= 2 D_i max_j |V_jc|; P.V adds eps_pv
     max_j |V_jc| (bf16x3 P and V: 3 * 2^-16, fp32 sums: T u) and ex2.approx 2^-21.  Times C_ATT = 4.
-    Mutations (the bound must reject them): `shift` relative positions, `drop_u`, `extra_key` (key T included)."""
+    Mutations (the bound must reject them): `shift` relative positions, `drop_u`, `extra_key` (key T included).
+    e_qkv [rows, 3 d] / e_pp [2 tmax - 1, d]: bounds on the errors of the inputs (a chain of kernels).  They move score i, j
+    by <= (|e_q|.|k_j| + |qu|.e_k + |e_q|.|PP_ij| + |qv|.e_PP) / sqrt(hd); with D_i the row's largest such move, ctx moves by
+    <= 2 D_i sum_j p_ij |V_jc| + sum_j p_ij e_V,jc, added to the bound as it stands (first order)."""
     hd = d // H
     out = np.zeros((qkv.shape[0], d))
     bound = np.zeros((qkv.shape[0], d))
@@ -331,6 +339,15 @@ def ref_attention(qkv, pp, u, v, row_off, n_utt, d, H, tmax, math_mode, kernel, 
             D = eps_s * sa.max(axis=1, keepdims=True)
             vmax = np.abs(V[:T]).max(axis=0, keepdims=True)
             bound[r0:r1, cs] = 4.0 * (2 * D + eps_pv) * vmax
+            if e_qkv is not None:
+                eq = e_qkv[r0:r1, cs]
+                ek = e_qkv[r0:r0 + Tk, d + h * hd:d + (h + 1) * hd]
+                ev = e_qkv[r0:r0 + Tk, 2 * d + h * hd:2 * d + (h + 1) * hd]
+                gq = eq @ np.abs(PPh).T
+                if e_pp is not None:
+                    gq = gq + np.abs(qv) @ e_pp[:, cs].T
+                Din = (eq @ np.abs(k).T + np.abs(qu) @ ek.T + np.take_along_axis(gq, prow, axis=1)).max(axis=1, keepdims=True)
+                bound[r0:r1, cs] += 2 * Din / math.sqrt(hd) * (p @ np.abs(V)) + p @ ev
     return out, bound
 
 
@@ -552,11 +569,12 @@ def test_layernorm_bound_rejects_unbiased_variance(pkg):
 
 
 # ----------------------------------------------------------------------------------------------------------- dwconv
-def ref_dwconv(g, w_tap, bias, row_off, neighbour_pad=False):
+def ref_dwconv(g, w_tap, bias, row_off, neighbour_pad=False, e_in=None, w_rel=0.0):
     """float64 depthwise conv (k taps, zero padding inside each utterance) + folded bias, then SiLU -> (y, bound).
     The kernel: fma chain over the k taps from the bias: |err| <= (k + 1) u (sum |w g| + |b|); SiLU with expf is
     1.1-Lipschitz plus 8 u |y| (expf, the division, the product).  Times C_DW = 2.  neighbour_pad (mutation): taps outside the utterance read the
-    neighbouring rows instead of zeros."""
+    neighbouring rows instead of zeros.  A chain of kernels adds 1.1 sum_taps |w| e_in (input error bound e_in) and
+    1.1 w_rel (sum |w g| + |b|) (weights and bias off by w_rel relative, e.g. a rounded BatchNorm fold)."""
     ks, d = w_tap.shape
     half = ks // 2
     g64 = g.astype(np.float64)
@@ -567,6 +585,7 @@ def ref_dwconv(g, w_tap, bias, row_off, neighbour_pad=False):
         T = r1 - r0
         acc = np.tile(bias.astype(np.float64), (T, 1))
         aab = np.tile(np.abs(bias.astype(np.float64)), (T, 1))
+        prop = np.zeros((T, d))
         for j in range(ks):
             src = np.arange(T) + j - half
             ok = (src >= 0) & (src < T)
@@ -576,9 +595,13 @@ def ref_dwconv(g, w_tap, bias, row_off, neighbour_pad=False):
             tap[ok] = g64[r0 + src[ok]]
             acc += w_tap[j].astype(np.float64) * tap
             aab += np.abs(w_tap[j].astype(np.float64) * tap)
+            if e_in is not None:
+                etap = np.zeros((T, d))
+                etap[ok] = e_in[r0 + src[ok]]
+                prop += np.abs(w_tap[j].astype(np.float64)) * etap
         yy = acc * sig64(acc)
         y[r0:r1] = yy
-        bd[r0:r1] = 2.0 * (1.1 * (ks + 1) * U * aab + 8 * U * np.abs(yy))
+        bd[r0:r1] = 2.0 * (1.1 * (ks + 1) * U * aab + 8 * U * np.abs(yy)) + 1.1 * (prop + w_rel * aab)
     return y, bd
 
 
