@@ -332,7 +332,7 @@ typedef struct {
     const int32_t *tok0, *frame_base;      /* [n_utt] last token, absolute frame of the first row */
     int32_t cluster;                       /* 0 = the engine's choice, 2 / 4 = only that size (PK_ERR_INVALID if it does not fit) */
     int32_t max_ctas;                      /* 0 = every SM, else the SM count the launch plans for */
-    int32_t no_stage;                      /* 1: no staging tile, as PK_TDT_NO_STAGE */
+    int32_t no_stage;                      /* 1: no staging tile: weights that do not fit are read from L2 */
 } pk_tdt_hook_in;
 /* Outputs (every array guarded; NULL pointers are not fetched).  h, z and the keys are those of the LAST step: h_hi / h_lo
  * [L][2][n_utt][P] are both state planes of every layer (the step's new h sits in the plane the utterance's committed state

@@ -36,8 +36,6 @@ __global__ void __launch_bounds__(AttnCfg<HD, BQ, BKV>::THREADS)
 relpos_attention_kernel(const float *__restrict__ qkv, int ld_qkv, const int32_t *__restrict__ row_off,
                         const float *__restrict__ pp, int tmax, const float *__restrict__ bias_u,
                         const float *__restrict__ bias_v, int d_model, ActBuf out) {
-    pdl_wait();
-    pdl_trigger();
     using C = AttnCfg<HD, BQ, BKV>;
     extern __shared__ __align__(16) float sm[];
     float *Qu_t = sm;                      // [HD][LQ]
@@ -204,7 +202,7 @@ void launch_t(const float *qkv, int ld_qkv, const int32_t *row_off, int n_utt, i
         attr_set = true;
     }
     dim3 grid((max_T + BQ - 1) / BQ, n_heads, n_utt);
-    launch_pdl(relpos_attention_kernel<HD, BQ, BKV>, dim3(grid), dim3(C::THREADS), C::SMEM, st, qkv, ld_qkv, row_off, pp, tmax, bu,
+    relpos_attention_kernel<HD, BQ, BKV><<<dim3(grid), dim3(C::THREADS), C::SMEM, st>>>(qkv, ld_qkv, row_off, pp, tmax, bu,
                                                                            bv, d_model, out);
 }
 

@@ -26,8 +26,6 @@ constexpr int MHA_CH = 16;    // keys per softmax rescale
 template <int HD>
 __global__ void __launch_bounds__(MHA_BQ)
 mha_kernel(const float *__restrict__ qkv, int ld_qkv, const int32_t *__restrict__ row_off, int d_model, float scale, ActBuf out) {
-    pdl_wait();
-    pdl_trigger();
     static_assert(HD % 4 == 0, "float4 rows");
     constexpr int V4 = HD / 4;
     __shared__ __align__(16) float Ks[MHA_BK][HD];
@@ -124,8 +122,6 @@ template <bool SPLIT3>
 __global__ void __launch_bounds__(128)
 mha_tc_kernel(const float *__restrict__ q32, const bf16 *__restrict__ kv_hi, const bf16 *__restrict__ kv_lo, int ld_kv,
               const int32_t *__restrict__ row_off, int d_model, float scale, ActBuf out) {
-    pdl_wait();
-    pdl_trigger();
     constexpr int HD = 24;
     __shared__ __align__(16) bf16 Qs[2][TC_BQ][TC_LD];    // [hi | lo][row][dim], dims 24..31 zero
     __shared__ __align__(16) bf16 Ks[2][TC_BK][TC_LD];    // [hi | lo][key][dim]
@@ -280,7 +276,8 @@ bool launch_mha_attention(const float *qkv, int ld_qkv, const int32_t *row_off, 
     if (max_T <= 0) return true;
     const float scale = 1.0f / std::sqrt((float)head_dim);   // transformer.cpp:27
     dim3 grid((max_T + MHA_BQ - 1) / MHA_BQ, n_heads, n_utt);
-    return launch_pdl(mha_kernel<24>, grid, dim3(MHA_BQ), 0, st, qkv, ld_qkv, row_off, d_model, scale, out) == cudaSuccess;
+    mha_kernel<24><<<grid, dim3(MHA_BQ), 0, st>>>(qkv, ld_qkv, row_off, d_model, scale, out);
+    return cudaGetLastError() == cudaSuccess;
 }
 
 }  // namespace pk
@@ -293,9 +290,9 @@ bool launch_mha_attention_tc(const float *q32, const bf16 *kv_hi, const bf16 *kv
     if (max_T <= 0) return true;
     const float scale = 1.0f / std::sqrt((float)head_dim);   // transformer.cpp:27
     dim3 grid((max_T + TC_BQ - 1) / TC_BQ, n_heads, n_utt);
-    const cudaError_t ce = kv_lo ? launch_pdl(mha_tc_kernel<true>, grid, dim3(128), 0, st, q32, kv_hi, kv_lo, ld_kv, row_off, d_model, scale, out)
-                                 : launch_pdl(mha_tc_kernel<false>, grid, dim3(128), 0, st, q32, kv_hi, kv_lo, ld_kv, row_off, d_model, scale, out);
-    return ce == cudaSuccess;
+    if (kv_lo) mha_tc_kernel<true><<<grid, dim3(128), 0, st>>>(q32, kv_hi, kv_lo, ld_kv, row_off, d_model, scale, out);
+    else mha_tc_kernel<false><<<grid, dim3(128), 0, st>>>(q32, kv_hi, kv_lo, ld_kv, row_off, d_model, scale, out);
+    return cudaGetLastError() == cudaSuccess;
 }
 
 }  // namespace pk

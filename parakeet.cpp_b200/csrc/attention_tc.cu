@@ -102,8 +102,6 @@ relpos_attention_tc_kernel(const float *__restrict__ q32, const float *__restric
                            const bf16 *__restrict__ qkv_hi, const bf16 *__restrict__ qkv_lo, int ld_qkv,
                            const int32_t *__restrict__ row_off, const bf16 *__restrict__ pp_hi,
                            const bf16 *__restrict__ pp_lo, int tmax, int d_model, ActBuf out) {
-    pdl_wait();
-    pdl_trigger();
     extern __shared__ __align__(16) uint8_t smraw[];
     using SM = AttnSmem<HD, QS>;
     constexpr int LDS_ = SM::LDS_, KS = HD / 16, NBO = HD / 8, CH = HD / 8;   // k-steps, output n-blocks, 16 B chunks per row
@@ -397,7 +395,7 @@ static bool launch_attn_t(const float *q32, const float *pos_u, const float *pos
         attr = true;
     }
     dim3 grid((max_T + BQ - 1) / BQ, n_heads, n_utt);
-    launch_pdl(relpos_attention_tc_kernel<HD, QS>, dim3(grid), dim3(TCA_THREADS), sizeof(SM), st, q32, pos_u, pos_v, qkv_hi, qkv_lo, ld_qkv, row_off, pp_hi, pp_lo,
+    relpos_attention_tc_kernel<HD, QS><<<dim3(grid), dim3(TCA_THREADS), sizeof(SM), st>>>(q32, pos_u, pos_v, qkv_hi, qkv_lo, ld_qkv, row_off, pp_hi, pp_lo,
                                                                               tmax, d_model, out);
     return true;
 }

@@ -17,8 +17,6 @@ namespace {
 __global__ void __launch_bounds__(256)
 ctc_frame_argmax_kernel(const float *__restrict__ logits, int M, int V, int ld, int32_t *__restrict__ best,
                         float *__restrict__ conf, float *__restrict__ logprobs) {
-    pdl_wait();
-    pdl_trigger();
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (row >= M) return;
@@ -91,8 +89,6 @@ __global__ void ctc_collapse_kernel(const int32_t *__restrict__ best, const floa
                                     int32_t *__restrict__ tok /* [n_utt][1+cap] */,
                                     int32_t *__restrict__ t_start, int32_t *__restrict__ t_end,
                                     float *__restrict__ t_conf) {
-    pdl_wait();
-    pdl_trigger();
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b < n_utt) ctc_collapse_row(best, conf, row_off, b, blank, cap, tok, t_start, t_end, t_conf);
 }
@@ -109,8 +105,6 @@ ctc_boosted_decode_kernel(const float *__restrict__ logprobs, const int32_t *__r
                           const int32_t *__restrict__ row_off, int V, int blank, int cap,
                           DeviceTrie all_rows, int32_t *__restrict__ tok, int32_t *__restrict__ t_start,
                           int32_t *__restrict__ t_end, float *__restrict__ t_conf) {
-    pdl_wait();
-    pdl_trigger();
     extern __shared__ uint32_t bsm[];
     const int W = (V + 31) >> 5;
     uint32_t *bits = bsm;                                   // [W]
@@ -224,19 +218,19 @@ void launch_ctc_boosted_decode(const float *logprobs, const int32_t *best, const
                                const DeviceTrie &trie, int32_t *tok, int32_t *t_start, int32_t *t_end, float *t_conf,
                                cudaStream_t st) {
     const size_t smem = sizeof(uint32_t) * ((V + 31) / 32) + sizeof(int) * 2 * BOOST_MAX_ACTIVE;
-    launch_pdl(ctc_boosted_decode_kernel, dim3(n_utt), dim3(256), smem, st, logprobs, best, conf, row_off, V, blank, cap, trie, tok, t_start, t_end, t_conf);
+    ctc_boosted_decode_kernel<<<dim3(n_utt), dim3(256), smem, st>>>(logprobs, best, conf, row_off, V, blank, cap, trie, tok, t_start, t_end, t_conf);
 }
 
 void launch_ctc_frame_argmax(const float *logits, int M, int V, int ld, int32_t *best, float *conf,
                              float *logprobs, cudaStream_t st) {
     if (M <= 0) return;
-    launch_pdl(ctc_frame_argmax_kernel, dim3((M + 7) / 8), dim3(256), 0, st, logits, M, V, ld, best, conf, logprobs);
+    ctc_frame_argmax_kernel<<<dim3((M + 7) / 8), dim3(256), 0, st>>>(logits, M, V, ld, best, conf, logprobs);
 }
 
 void launch_ctc_collapse(const int32_t *best, const float *conf, const int32_t *row_off, int n_utt, int blank,
                          int cap, int32_t *tok, int32_t *t_start, int32_t *t_end, float *t_conf,
                          cudaStream_t st) {
-    launch_pdl(ctc_collapse_kernel, dim3((n_utt + 63) / 64), dim3(64), 0, st, best, conf, row_off, n_utt, blank, cap, tok, t_start,
+    ctc_collapse_kernel<<<dim3((n_utt + 63) / 64), dim3(64), 0, st>>>(best, conf, row_off, n_utt, blank, cap, tok, t_start,
                                                         t_end, t_conf);
 }
 

@@ -25,8 +25,6 @@ __global__ void __launch_bounds__(CTC_ALIGN_THREADS)
 ctc_align_kernel(const float *__restrict__ logprobs, const int32_t *__restrict__ row_off, int V, const int32_t *__restrict__ tgt,
                  const int32_t *__restrict__ tgt_off, uint8_t *__restrict__ bp, int bp_stride, int32_t *__restrict__ best,
                  float *__restrict__ conf, double *__restrict__ score, double *__restrict__ loglik, int32_t *__restrict__ path) {
-    pdl_wait();
-    pdl_trigger();
     extern __shared__ double dsm[];
     __shared__ int s_rep;
     const int b = blockIdx.x, tid = threadIdx.x;
@@ -113,7 +111,7 @@ void launch_ctc_align(const float *logprobs, const int32_t *row_off, int n_utt, 
         cudaFuncSetAttribute(ctc_align_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         attr_set = true;
     }
-    launch_pdl(ctc_align_kernel, dim3(n_utt), dim3(CTC_ALIGN_THREADS), smem, st, logprobs, row_off, V, tgt, tgt_off, bp, bp_stride,
+    ctc_align_kernel<<<dim3(n_utt), dim3(CTC_ALIGN_THREADS), smem, st>>>(logprobs, row_off, V, tgt, tgt_off, bp, bp_stride,
                best, conf, score, loglik, path);
 }
 

@@ -25,8 +25,6 @@ constexpr int PER_LANE = (MAX_CAND / NWARP + 31) / 32;   // candidates a lane sc
 __global__ void __launch_bounds__(256)
 ctc_frame_topk_kernel(const float *__restrict__ logprobs, int M, int V, int W, int32_t *__restrict__ topk_id,
                       float *__restrict__ topk_lp, float *__restrict__ blank_lp) {
-    pdl_wait();
-    pdl_trigger();
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (row >= M) return;
@@ -120,8 +118,6 @@ ctc_beam_kernel(const float *__restrict__ logprobs, const int32_t *__restrict__ 
                 const float *__restrict__ blank_lp, const int32_t *__restrict__ row_off, int V, int W, int cap, DeviceLM lm,
                 DevicePieces pc, int32_t *__restrict__ bp, int32_t *__restrict__ tok, int32_t *__restrict__ t_start,
                 int32_t *__restrict__ t_end, float *__restrict__ t_conf) {
-    pdl_wait();
-    pdl_trigger();
     __shared__ BeamSet bs[2];
     __shared__ double c_sc[MAX_CAND];                  // candidate scores: [blank/repeat of beam j][extension (i, r) at nb + i W + r]
     __shared__ double n_pb[BEAM_MAX], n_pnb[BEAM_MAX], w_sc[BEAM_MAX];
@@ -431,13 +427,13 @@ std::string ctc_beam_tables(const pk_lm *lm, const pk_vocab *vocab, int V, const
 void launch_ctc_frame_topk(const float *logprobs, int M, int V, int width, int32_t *topk_id, float *topk_lp, float *blank_lp,
                            cudaStream_t st) {
     if (M <= 0) return;
-    launch_pdl(ctc_frame_topk_kernel, dim3((M + 7) / 8), dim3(256), 0, st, logprobs, M, V, width, topk_id, topk_lp, blank_lp);
+    ctc_frame_topk_kernel<<<dim3((M + 7) / 8), dim3(256), 0, st>>>(logprobs, M, V, width, topk_id, topk_lp, blank_lp);
 }
 
 void launch_ctc_beam(const float *logprobs, const int32_t *topk_id, const float *topk_lp, const float *blank_lp,
                      const int32_t *row_off, int n_utt, int V, int width, int cap, const DeviceLM &lm, const DevicePieces &pieces,
                      int32_t *bp, int32_t *tok, int32_t *t_start, int32_t *t_end, float *t_conf, cudaStream_t st) {
-    launch_pdl(ctc_beam_kernel, dim3(n_utt), dim3(CTC_BEAM_THREADS), 0, st, logprobs, topk_id, topk_lp, blank_lp, row_off, V, width,
+    ctc_beam_kernel<<<dim3(n_utt), dim3(CTC_BEAM_THREADS), 0, st>>>(logprobs, topk_id, topk_lp, blank_lp, row_off, V, width,
                cap, lm, pieces, bp, tok, t_start, t_end, t_conf);
 }
 

@@ -18,6 +18,7 @@
 #include "engine.h"
 
 #include <algorithm>
+#include <cstdlib>
 #include <unordered_map>
 
 namespace pk_detail {
@@ -1067,9 +1068,7 @@ static pk_status create_engine(const pk_config &c, const pk_sortformer_config *s
         // every row through the same GEMM kernel whatever the batch: an utterance's activities do not depend on its batch
         e->skinny = false;
     }
-    if (const char *ev = getenv("PK_GRAPH")) e->use_graphs = atoi(ev) != 0;
     if (const char *ev = getenv("PK_ATTN_TC")) e->attn_tc = atoi(ev) != 0;
-    if (const char *ev = getenv("PK_GEMM_SKINNY")) e->skinny = e->stream_skinny = atoi(ev) != 0;
     if (const char *ev = getenv("PK_GEMM_CLUSTER")) e->gemm_cluster = atoi(ev);
     e->device = device;
     if (cudaSetDevice(device) != cudaSuccess) {

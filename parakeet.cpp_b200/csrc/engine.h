@@ -304,9 +304,8 @@ struct pk_engine {
     pk_status gemm_ln(const Act &A, int lda, const GemmWeight &W, int M_, bool resid_in_x, float alpha, const float *ln1_w, const float *ln1_b,
                       bool out_ln1, const float *ln2_w, const float *ln2_b, ActBuf planes);
     int gemm_cluster = 0;                      // PK_GEMM_CLUSTER=2|4: wide GEMMs (fc1, q/k/v, pw1) run as clusters of 2 | 4 CTAs along N with the A tile multicast
-    // few-row GEMMs (M <= 128: streaming steps, short utterances) go to gemm_skinny.cu (PK_GEMM_SKINNY=0: never)
+    // few-row GEMMs (M <= 128: streaming steps, short utterances) go to gemm_skinny.cu (offline diarization keeps it off)
     bool skinny = true;
-    bool stream_skinny = true;                 // the same for the steps of Sortformer streams (offline diarization keeps skinny off)
     float *skinny_ws = nullptr;
     size_t skinny_ws_floats = 0;
     unsigned int *skinny_tickets = nullptr;

@@ -19,8 +19,6 @@ constexpr int BM = 128, BN = 128, BK = 16;
 __global__ void __launch_bounds__(256)
 gemm_simt_kernel(const float *__restrict__ A, int lda, const float *__restrict__ W, int ldw, int M, int N,
                  int K, EpiParams epi) {
-    pdl_wait();
-    pdl_trigger();
     __shared__ __align__(16) float As[2][BK][BM + 4];
     __shared__ __align__(16) float Bs[2][BK][BN + 4];
     const int tid = threadIdx.x;
@@ -101,7 +99,7 @@ void launch_gemm_simt(const float *A, int lda, const float *W, int ldw, int M, i
                       const EpiParams &epi, cudaStream_t st) {
     if (M <= 0 || N <= 0) return;
     dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
-    launch_pdl(gemm_simt_kernel, dim3(grid), dim3(256), 0, st, A, lda, W, ldw, M, N, K, epi);
+    gemm_simt_kernel<<<dim3(grid), dim3(256), 0, st>>>(A, lda, W, ldw, M, N, K, epi);
 }
 
 }  // namespace pk

@@ -38,8 +38,6 @@ __global__ void __launch_bounds__(SK_THREADS, 2)
 gemm_skinny_kernel(const bf16 *__restrict__ Ahi, const bf16 *__restrict__ Alo, int lda, const bf16 *__restrict__ Whi,
                    const bf16 *__restrict__ Wlo, int M, int N, int K, int kc_chunks /* 64-wide chunks per K slice */,
                    float *__restrict__ ws, unsigned int *__restrict__ tickets, const __grid_constant__ EpiParams epi) {
-    pdl_wait();
-    pdl_trigger();
     extern __shared__ __align__(16) uint8_t sk_raw[];
     bf16 *stage = reinterpret_cast<bf16 *>(sk_raw);            // [2 stages][A_hi | A_lo | W_hi | W_lo]
     constexpr int STAGE_ELEMS = 2 * (SK_A_ELEMS + SK_W_ELEMS);
@@ -191,9 +189,9 @@ cudaError_t launch_gemm_skinny(const bf16 *Ahi, const bf16 *Alo, int lda, const 
     }
     dim3 grid(ntiles, nsplit);
     if (split3)
-        launch_pdl(gemm_skinny_kernel<true>, dim3(grid), dim3(SK_THREADS), SK_SMEM, st, Ahi, Alo, lda, Whi, Wlo, M, N, K, chunks / nsplit, ws, tickets, epi);
+        gemm_skinny_kernel<true><<<grid, dim3(SK_THREADS), SK_SMEM, st>>>(Ahi, Alo, lda, Whi, Wlo, M, N, K, chunks / nsplit, ws, tickets, epi);
     else
-        launch_pdl(gemm_skinny_kernel<false>, dim3(grid), dim3(SK_THREADS), SK_SMEM, st, Ahi, Alo, lda, Whi, Wlo, M, N, K, chunks / nsplit, ws, tickets, epi);
+        gemm_skinny_kernel<false><<<grid, dim3(SK_THREADS), SK_SMEM, st>>>(Ahi, Alo, lda, Whi, Wlo, M, N, K, chunks / nsplit, ws, tickets, epi);
     return cudaGetLastError();
 }
 

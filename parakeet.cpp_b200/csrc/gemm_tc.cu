@@ -388,8 +388,6 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap &tmA_hi, const CU
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     cluster_sync();      // every CTA's barriers exist before a peer multicasts into it / arrives on them
-    pdl_wait();      // barriers are set up while the previous grid drains; now its results are visible
-    pdl_trigger();
 
     if (wg == 0) {
         // ===================== TMA producer =====================
@@ -412,7 +410,6 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap &tmA_hi, const CU
                     if (NPASS == 3) tma_load_2d(st + 2 * C::A_BYTES + C::W_BYTES, &tmW_lo, &full[s], kb * BK, n0);
                 }
             }
-            pdl_trigger_late();     // every operand load of this CTA has been issued
         }
         __syncwarp();                // the elected lane rejoins its warp before the .aligned cluster barrier at the end
     } else {
@@ -502,8 +499,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    pdl_wait();      // barriers are set up while the previous grid drains; now its results are visible
-    pdl_trigger();
 
     if (wg == 0) {
         // ===================== TMA producer =====================
@@ -524,7 +519,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
                     if (NPASS == 3) tma_load_2d(st + 2 * C::A_BYTES + C::W_BYTES, &tmW_lo, &full[s], kb * BK, n0);
                 }
             }
-            pdl_trigger_late();     // every operand load of this CTA has been issued
         }
     } else {
         // ===================== consumers: wgmma + epilogue, one whole tile each =====================
@@ -693,7 +687,7 @@ cudaError_t launch_k(const TcOperand &A, const TcOperand &W, int M, int N, int K
     const int num_tiles = ((N + BN - 1) / BN) * ((M + BM - 1) / BM);
     dim3 grid(num_tiles < num_sms ? num_tiles : num_sms);
     const CUtensorMap &alo = (NPASS == 3) ? A.lo : A.hi, &wlo = (NPASS == 3) ? W.lo : W.hi;
-    launch_pdl(gemm_tc_kernel<BN, NPASS, EK, STAGED>, dim3(grid), dim3(TC_THREADS), C::SMEM, st, A.hi, alo, W.hi, wlo, M, N, K, epi, om);
+    gemm_tc_kernel<BN, NPASS, EK, STAGED><<<grid, dim3(TC_THREADS), C::SMEM, st>>>(A.hi, alo, W.hi, wlo, M, N, K, epi, om);
     return cudaGetLastError();
 }
 
@@ -748,7 +742,8 @@ cudaError_t launch_kcl(const TcOperand &A_sl, const TcOperand &W, int M, int N, 
     if (ncl > num_sms / CL) ncl = num_sms / CL;
     if (ncl > units) ncl = units;
     const CUtensorMap &alo = (NPASS == 3) ? A_sl.lo : A_sl.hi, &wlo = (NPASS == 3) ? W.lo : W.hi;
-    return launch_pdl(gemm_tc_cl_kernel<NPASS, EK, CL>, dim3((unsigned)(ncl * CL)), dim3(TC_THREADS), C::SMEM, st, A_sl.hi, alo, W.hi, wlo, M, N, K, epi);
+    gemm_tc_cl_kernel<NPASS, EK, CL><<<dim3((unsigned)(ncl * CL)), dim3(TC_THREADS), C::SMEM, st>>>(A_sl.hi, alo, W.hi, wlo, M, N, K, epi);
+    return cudaGetLastError();
 }
 
 }  // namespace

@@ -317,12 +317,11 @@ struct TdtParams {
 // Geometry controls of one decode launch (kernel tests only) and the geometry the launch chose.
 struct TdtLaunchCtl {
     int cluster = 0;          // in: 0 = the engine's choice, 2 / 4 = only that cluster size (no fallback)
-    bool no_stage = false;    // in: no staging tile (as PK_TDT_NO_STAGE): weights that do not fit are read from L2
+    bool no_stage = false;    // in: no staging tile: weights that do not fit are read from L2
     int grid = 0, CL = 0, UPC = 0, OPC = 0;                    // out (grid = 0: nothing was launched)
     int out_in_smem = 0, wih_in_smem = 0, staged_ih = 0, wstage_rows = 0;   // out; staged_ih as decided by cluster 0
 };
-// ctl = nullptr: the engine's choice (PK_TDT_CLUSTER = 2 forces the 2-CTA cluster), decided per launch from the shapes
-// and the occupancy query.
+// ctl = nullptr: the engine's choice, decided per launch from the shapes and the occupancy query.
 cudaError_t launch_tdt_decode(TdtParams p, int num_sms, cudaStream_t st, TdtLaunchCtl *ctl = nullptr);
 // gate-major LSTM weight [4P][P] (gate order i, f, g, o) -> unit-major [4P][P] (row = unit*4 + gate), the row order
 // tdt_decode_kernel expects

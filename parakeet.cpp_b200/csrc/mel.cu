@@ -72,8 +72,6 @@ __global__ void __launch_bounds__(WARPS * 32)
 mel_logpower_kernel(const float *__restrict__ pcm, const int64_t *__restrict__ pcm_off,
                     const int32_t *__restrict__ frame_off, const int32_t *__restrict__ n_frames_arr, int n_mels, MelTables tb,
                     float *__restrict__ logmel) {
-    pdl_wait();
-    pdl_trigger();
     extern __shared__ float smem[];
     // layout: [window 400][tw256 512][tw512 514][fb weights nnz][per-warp: frame 512 | Z 512 | P 260]
     float *s_win = smem;
@@ -209,8 +207,6 @@ __device__ __forceinline__ void mel_chunk(int c, int F, int &f0, int &f1) {
 
 __global__ void mel_stats_kernel(const float *__restrict__ logmel, const int32_t *__restrict__ frame_off, int n_mels,
                                  float *__restrict__ part /* [utterance][MEL_CH][2][n_mels] */) {
-    pdl_wait();
-    pdl_trigger();
     extern __shared__ float red[];  // [groups][n_mels]
     const int b = blockIdx.y, c = blockIdx.x;
     const int groups = blockDim.x / n_mels;
@@ -251,8 +247,6 @@ __global__ void mel_stats_kernel(const float *__restrict__ logmel, const int32_t
 
 __global__ void mel_apply_kernel(const float *__restrict__ logmel, const int32_t *__restrict__ frame_off, int n_mels,
                                  const float *__restrict__ part, float *__restrict__ feats) {
-    pdl_wait();
-    pdl_trigger();
     const int b = blockIdx.y, c = blockIdx.x;
     const int groups = blockDim.x / n_mels;
     const int m = threadIdx.x % n_mels, g = threadIdx.x / n_mels;
@@ -344,19 +338,19 @@ void launch_mel(const float *pcm, const int64_t *pcm_off, const int32_t *frame_o
                 int max_frames, int n_mels, const MelTables &tb, float *logmel, float *feats, float *part,
                 cudaStream_t st, bool normalize) {
     dim3 grid((max_frames + WARPS * 4 - 1) / (WARPS * 4), n_utt);
-    launch_pdl(mel_logpower_kernel<false>, dim3(grid), dim3(WARPS * 32), mel_smem_bytes(tb), st, pcm, pcm_off, frame_off, nullptr, n_mels, tb,
+    mel_logpower_kernel<false><<<dim3(grid), dim3(WARPS * 32), mel_smem_bytes(tb), st>>>(pcm, pcm_off, frame_off, nullptr, n_mels, tb,
                                                                              normalize ? logmel : feats);
     if (!normalize) return;
     int groups = MEL_NORM_THREADS / n_mels;  // 8 for 80 bins, 5 for 128
-    launch_pdl(mel_stats_kernel, dim3(MEL_CH, n_utt), dim3(groups * n_mels), sizeof(float) * groups * n_mels, st, logmel, frame_off, n_mels, part);
-    launch_pdl(mel_apply_kernel, dim3(MEL_CH, n_utt), dim3(groups * n_mels), 0, st, logmel, frame_off, n_mels, part, feats);
+    mel_stats_kernel<<<dim3(MEL_CH, n_utt), dim3(groups * n_mels), sizeof(float) * groups * n_mels, st>>>(logmel, frame_off, n_mels, part);
+    mel_apply_kernel<<<dim3(MEL_CH, n_utt), dim3(groups * n_mels), 0, st>>>(logmel, frame_off, n_mels, part, feats);
 }
 
 void launch_mel_stream(const float *sig, const int64_t *sig_off, const int32_t *n_frames, const int32_t *out_row, int n_streams,
                        int max_frames, int n_mels, const MelTables &tb, float *logmel, cudaStream_t st) {
     if (max_frames <= 0) return;
     dim3 grid((max_frames + WARPS * 4 - 1) / (WARPS * 4), n_streams);
-    launch_pdl(mel_logpower_kernel<true>, dim3(grid), dim3(WARPS * 32), mel_smem_bytes(tb), st, sig, sig_off, out_row, n_frames, n_mels, tb, logmel);
+    mel_logpower_kernel<true><<<dim3(grid), dim3(WARPS * 32), mel_smem_bytes(tb), st>>>(sig, sig_off, out_row, n_frames, n_mels, tb, logmel);
 }
 
 }  // namespace pk

@@ -42,8 +42,6 @@ __global__ void __launch_bounds__(256)
 layernorm_kernel(const float *__restrict__ x, int M, int d, const float *__restrict__ w1,
                  const float *__restrict__ b1, float *out1_f32, ActBuf out1_act,
                  const float *__restrict__ w2, const float *__restrict__ b2, ActBuf out2_act, float eps) {
-    pdl_wait();
-    pdl_trigger();
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (row >= M) return;
@@ -95,8 +93,6 @@ __global__ void __launch_bounds__(128)
 dwconv_bn_silu_kernel(const float *__restrict__ g, const int32_t *__restrict__ row_off, int d,
                       const float *__restrict__ w /* tap-major [KS][d], BatchNorm folded */, const float *__restrict__ bias /* [d] folded */,
                       ActBuf out) {
-    pdl_wait();
-    pdl_trigger();
     const int b = blockIdx.z;
     const int r0 = row_off[b], T = row_off[b + 1] - r0;
     const int t0 = blockIdx.y * DW_TT;
@@ -135,8 +131,6 @@ dwconv_bn_silu_kernel(const float *__restrict__ g, const int32_t *__restrict__ r
 }
 
 __global__ void split_kernel(const float *__restrict__ x, size_t n4, ActBuf out) {
-    pdl_wait();
-    pdl_trigger();
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n4) store_act4(out, i * 4, reinterpret_cast<const float4 *>(x)[i]);
 }
@@ -146,14 +140,14 @@ __global__ void split_kernel(const float *__restrict__ x, size_t n4, ActBuf out)
 void launch_split(const float *x, size_t n, ActBuf out, cudaStream_t st) {
     const size_t n4 = n / 4;
     if (n4 == 0) return;
-    launch_pdl(split_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, st, x, n4, out);
+    split_kernel<<<dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, st>>>(x, n4, out);
 }
 
 void launch_layernorm(const float *x, int M, int d, const float *w1, const float *b1, float *out1_f32,
                       ActBuf out1_act, const float *w2, const float *b2, ActBuf out2_act, cudaStream_t st) {
     if (M <= 0) return;
     const int warps = 8;
-    launch_pdl(layernorm_kernel, dim3((M + warps - 1) / warps), dim3(warps * 32), 0, st, x, M, d, w1, b1, out1_f32, out1_act, w2, b2,
+    layernorm_kernel<<<dim3((M + warps - 1) / warps), dim3(warps * 32), 0, st>>>(x, M, d, w1, b1, out1_f32, out1_act, w2, b2,
                                                                      out2_act, 1e-5f);
 }
 
@@ -162,7 +156,7 @@ bool launch_dwconv_bn_silu(const float *g, const int32_t *row_off, int n_utt, in
     if (ks != 9) return false;
     dim3 block(128);
     dim3 grid((d / 4 + 127) / 128, (max_T + DW_TT - 1) / DW_TT, n_utt);
-    launch_pdl(dwconv_bn_silu_kernel<9>, dim3(grid), dim3(block), 0, st, g, row_off, d, w, bias, out);
+    dwconv_bn_silu_kernel<9><<<dim3(grid), dim3(block), 0, st>>>(g, row_off, d, w, bias, out);
     return true;
 }
 

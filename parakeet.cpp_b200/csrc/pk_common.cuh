@@ -3,59 +3,10 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
-#include <utility>
 
 namespace pk {
 
 typedef __nv_bfloat16 bf16;
-
-// ---------------------------------------------------------------- programmatic dependent launch
-// Every kernel of the path starts with pdl_wait() (griddepcontrol.wait: returns once the preceding grid has completed and
-// its writes are visible; a no-op for a normal launch) and is launched through launch_pdl(); with PK_PDL=1 the launch
-// carries programmatic stream serialisation, so the next grid's CTAs are scheduled and do their input-independent set-up
-// (barrier init, index math) while the previous grid drains.  Because EVERY kernel waits before its
-// first global access, completion of a grid still implies completion of all its predecessors.
-// The attribute is OFF by default (PK_PDL=1 turns it on): inside the CUDA graphs the product path replays, graph edges
-// are already cheap.
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-#ifndef PK_PDL_TRIGGER
-#define PK_PDL_TRIGGER 1     // 0: implicit (at CTA exit); 1: at the top of every kernel; 2: only late in the GEMM (all loads issued)
-#endif
-__device__ __forceinline__ void pdl_trigger() {
-#if PK_PDL_TRIGGER == 1
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-#endif
-}
-__device__ __forceinline__ void pdl_trigger_late() {
-#if PK_PDL_TRIGGER == 2
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-#endif
-}
-
-inline int pdl_enabled() {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("PK_PDL");
-        v = (e && e[0] == '1') ? 1 : 0;
-    }
-    return v;
-}
-
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args &&...args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = pdl_enabled();
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kern, KArgs(std::forward<Args>(args))...);
-}
 
 // cudaFuncSetAttribute is per DEVICE: a process that drives several GPUs (one pk_engine per device, e.g.
 // examples/sharded_transcribe.cpp) must set a kernel's attributes once on each of them.  Returns the flag of the

@@ -88,8 +88,6 @@ const RateTable &table_for(int src_rate, int dst_rate) {
 __global__ void polyphase_resample_kernel(const float *__restrict__ in, const int64_t *__restrict__ in_off,
                                           const int64_t *__restrict__ out_off, const double *__restrict__ table, int up, int down,
                                           float *__restrict__ out) {
-    pdl_wait();
-    pdl_trigger();
     const int b = blockIdx.y;
     const float *x = in + in_off[b];
     const int64_t n = in_off[b + 1] - in_off[b], m = out_off[b + 1] - out_off[b];
@@ -146,7 +144,7 @@ bool launch_resample(const float *in, const int64_t *in_off, const int64_t *out_
     int64_t bx = (max_out + threads - 1) / threads;
     if (bx > 4096) bx = 4096;
     if (bx < 1) bx = 1;
-    launch_pdl(polyphase_resample_kernel, dim3(dim3((unsigned)bx, n_utt)), dim3(threads), 0, st, in, in_off, out_off, tab, up, down, out);
+    polyphase_resample_kernel<<<dim3((unsigned)bx, n_utt), dim3(threads), 0, st>>>(in, in_off, out_off, tab, up, down, out);
     return cudaGetLastError() == cudaSuccess;
 }
 

@@ -15,8 +15,6 @@ __global__ void __launch_bounds__(256)
 speaker_head_kernel(const float *__restrict__ x, int M, int D, int S, const float *__restrict__ w1t /* [D][D] = W1^T */,
                     const float *__restrict__ b1, const float *__restrict__ w2 /* [S][D] */, const float *__restrict__ b2,
                     float *__restrict__ probs) {
-    pdl_wait();
-    pdl_trigger();
     extern __shared__ __align__(16) float sm[];
     float *W1 = sm;                    // [D][D]
     float *W2 = W1 + (size_t)D * D;    // [S][D]
@@ -73,7 +71,8 @@ bool launch_speaker_head(const float *x, int M, int D, int S, const float *w1t, 
     }
     const int tiles = (M + HEAD_R - 1) / HEAD_R;
     const int grid = std::max(1, std::min(tiles, num_sms));
-    return launch_pdl(speaker_head_kernel, dim3(grid), dim3(D), smem, st, x, M, D, S, w1t, b1, w2, b2, probs) == cudaSuccess;
+    speaker_head_kernel<<<dim3(grid), dim3(D), smem, st>>>(x, M, D, S, w1t, b1, w2, b2, probs);
+    return cudaGetLastError() == cudaSuccess;
 }
 
 }  // namespace pk

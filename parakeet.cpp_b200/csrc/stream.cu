@@ -17,8 +17,6 @@ namespace {
 //         mel_in = [leftover mel frames | (new frames, written by the mel kernel)]
 __global__ void stream_prep_kernel(const float *__restrict__ chunk, const StreamPlan *__restrict__ plan, StreamState st,
                                    float *__restrict__ ssig, float *__restrict__ mel_in, int n_mels) {
-    pdl_wait();
-    pdl_trigger();
     const int s = blockIdx.x;
     const StreamPlan p = plan[s];
     const float *x = chunk + p.chunk_off;
@@ -46,8 +44,6 @@ __global__ void stream_prep_kernel(const float *__restrict__ chunk, const Stream
 __global__ void stream_post_kernel(const float *__restrict__ chunk, const StreamPlan *__restrict__ plan, StreamState st,
                                    const float *__restrict__ ssig, const float *__restrict__ mel_in, int n_mels,
                                    float *__restrict__ feats) {
-    pdl_wait();
-    pdl_trigger();
     const int s = blockIdx.x;
     const StreamPlan p = plan[s];
     const float *sig = ssig + p.sig_off;
@@ -71,8 +67,6 @@ __global__ void stream_post_kernel(const float *__restrict__ chunk, const Stream
 // first `take` rows go to the packed encoder input, the rest (< 8) back into the queue.
 __global__ void diar_stream_join_kernel(const StreamPlan *__restrict__ plan, const float *__restrict__ mel_new,
                                         float *__restrict__ melq, int n_mels, float *__restrict__ feats) {
-    pdl_wait();
-    pdl_trigger();
     const int s = blockIdx.x;
     const StreamPlan p = plan[s];
     float *q = melq + (size_t)s * 8 * n_mels;
@@ -103,8 +97,6 @@ stream_attention_kernel(const float *__restrict__ qkv, int ld_qkv, const int32_t
                         const int32_t *__restrict__ ring_start, float *__restrict__ kc, float *__restrict__ vc,
                         int L, int hd, int d_model, const float *__restrict__ pp, int tmax,
                         const float *__restrict__ bu, const float *__restrict__ bv, ActBuf out) {
-    pdl_wait();
-    pdl_trigger();
     extern __shared__ float sm[];
     const int h = blockIdx.x, a = blockIdx.y, s = act_stream[a];
     const int r0 = row_off[a], C = row_off[a + 1] - r0;
@@ -184,8 +176,6 @@ template <int KS>
 __global__ void stream_dwconv_kernel(const float *__restrict__ glu, const int32_t *__restrict__ row_off,
                                      const int32_t *__restrict__ act_stream, float *__restrict__ cache, int d,
                                      const float *__restrict__ w, const float *__restrict__ bias, ActBuf out) {
-    pdl_wait();
-    pdl_trigger();
     const int a = blockIdx.x, s = act_stream[a];
     const int r0 = row_off[a], C = row_off[a + 1] - r0;
     float *cs = cache + (size_t)s * (KS - 1) * d;
@@ -216,16 +206,16 @@ __global__ void stream_dwconv_kernel(const float *__restrict__ glu, const int32_
 
 void launch_stream_prep(const float *chunk, const StreamPlan *plan, StreamState st, int n_streams, float *ssig, float *mel_in,
                         int n_mels, cudaStream_t s) {
-    launch_pdl(stream_prep_kernel, dim3(n_streams), dim3(256), 0, s, chunk, plan, st, ssig, mel_in, n_mels);
+    stream_prep_kernel<<<dim3(n_streams), dim3(256), 0, s>>>(chunk, plan, st, ssig, mel_in, n_mels);
 }
 void launch_stream_post(const float *chunk, const StreamPlan *plan, StreamState st, int n_streams, const float *ssig,
                         const float *mel_in, int n_mels, float *feats, cudaStream_t s) {
-    launch_pdl(stream_post_kernel, dim3(n_streams), dim3(256), 0, s, chunk, plan, st, ssig, mel_in, n_mels, feats);
+    stream_post_kernel<<<dim3(n_streams), dim3(256), 0, s>>>(chunk, plan, st, ssig, mel_in, n_mels, feats);
 }
 
 void launch_diar_stream_join(const StreamPlan *plan, const float *mel_new, float *melq, int n_streams, int n_mels, float *feats,
                              cudaStream_t s) {
-    launch_pdl(diar_stream_join_kernel, dim3(n_streams), dim3(256), 0, s, plan, mel_new, melq, n_mels, feats);
+    diar_stream_join_kernel<<<dim3(n_streams), dim3(256), 0, s>>>(plan, mel_new, melq, n_mels, feats);
 }
 
 size_t stream_attention_smem(int L, int Cmax, int hd) { return sizeof(float) * ((size_t)2 * (L + Cmax) * (hd + 1) + 2 * hd + L + Cmax); }
@@ -242,7 +232,7 @@ bool launch_stream_attention(const float *qkv, int ld_qkv, const int32_t *row_of
         if (cudaFuncSetAttribute(stream_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return false;
         attr = smem;
     }
-    launch_pdl(stream_attention_kernel, dim3(dim3(n_heads, n_active)), dim3(128), smem, s, qkv, ld_qkv, row_off, act_stream, cache_len, ring_start, kc, vc,
+    stream_attention_kernel<<<dim3(n_heads, n_active), dim3(128), smem, s>>>(qkv, ld_qkv, row_off, act_stream, cache_len, ring_start, kc, vc,
                                                                       L, hd, d_model, pp, tmax, bu, bv, out);
     return true;
 }
@@ -250,7 +240,7 @@ bool launch_stream_attention(const float *qkv, int ld_qkv, const int32_t *row_of
 bool launch_stream_dwconv(const float *glu, const int32_t *row_off, const int32_t *act_stream, int n_active, float *cache, int d,
                           int ks, const float *w, const float *bias, ActBuf out, cudaStream_t s) {
     if (ks != 9) return false;
-    launch_pdl(stream_dwconv_kernel<9>, dim3(n_active), dim3(256), 0, s, glu, row_off, act_stream, cache, d, w, bias, out);
+    stream_dwconv_kernel<9><<<dim3(n_active), dim3(256), 0, s>>>(glu, row_off, act_stream, cache, d, w, bias, out);
     return true;
 }
 

@@ -615,7 +615,7 @@ pk_status diar_stream_step(pk_engine *e, const float *pcm, const int64_t *offset
     if ((ps = e->upload_shapes())) return ps;
     auto body = [e, enc_out, st]() -> pk_status {
         const bool sk = e->skinny;
-        e->skinny = e->stream_skinny;              // few rows per step: the weight-streaming GEMM
+        e->skinny = true;                          // few rows per step: the weight-streaming GEMM
         pk_status q = e->run_conv1();
         if (!q) q = e->run_subsample_tail();
         if (!q) q = e->run_stream_layers();

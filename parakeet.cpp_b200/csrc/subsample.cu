@@ -24,8 +24,6 @@ subsample_conv1_dw1_kernel(const float *__restrict__ feats, const int32_t *__res
                            const int32_t *__restrict__ s2_off, int mel, int C,
                            const float *__restrict__ w1, const float *__restrict__ b1,
                            const float *__restrict__ wd, const float *__restrict__ bd, ActBuf out) {
-    pdl_wait();
-    pdl_trigger();
     extern __shared__ float S[];  // [(4*TT2+3)][mel + 4], column index = col + 2
     const int b = blockIdx.y;
     const int F = frame_off[b + 1] - frame_off[b];
@@ -116,8 +114,6 @@ __global__ void subsample_dw_kernel(const float *__restrict__ in, const int32_t 
                                     const float *__restrict__ wd /* tap-major [9][C] */,
                                     const float *__restrict__ bd, ActBuf out, int total_out_rows,
                                     int n_utt) {
-    pdl_wait();
-    pdl_trigger();
     // one thread per (output row, 4 channels)
     const int c4n = C >> 2;
     const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -165,7 +161,7 @@ void launch_subsample_conv1_dw1(const float *feats, const int32_t *frame_off, co
     int threads = ((C + 31) / 32) * 32;
     if (threads > 256) threads = 256;            // the kernel strides over channels
     size_t smem = sizeof(float) * (4 * TT2 + 3) * (mel + 4);
-    launch_pdl(subsample_conv1_dw1_kernel, dim3(grid), dim3(threads), smem, st, feats, frame_off, s2_off, mel, C, w1, b1, wd, bd,
+    subsample_conv1_dw1_kernel<<<dim3(grid), dim3(threads), smem, st>>>(feats, frame_off, s2_off, mel, C, w1, b1, wd, bd,
                                                             out);
 }
 
@@ -174,7 +170,7 @@ void launch_subsample_dw(const float *in, const int32_t *in_rows, const int32_t 
                          const float *bd, ActBuf out, int total_out_rows, cudaStream_t st) {
     long long n = (long long)total_out_rows * (C / 4);
     int threads = 256;
-    launch_pdl(subsample_dw_kernel, dim3((unsigned)((n + threads - 1) / threads)), dim3(threads), 0, st, 
+    subsample_dw_kernel<<<dim3((unsigned)((n + threads - 1) / threads)), dim3(threads), 0, st>>>(
         in, in_rows, in_off, out_off, fin, C, wd, bd, out, total_out_rows, n_utt);
 }
 

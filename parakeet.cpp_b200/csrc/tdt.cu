@@ -53,7 +53,6 @@
 // and read A fragments with ldmatrix.  Operands of the phase epilogues (G0[token], EP[t], biases)
 // are fetched BEFORE the product so their L2 latency overlaps it; the LSTM cell state never leaves
 // shared memory.
-#include <cstdlib>
 #include <cstring>
 #include <map>
 
@@ -821,8 +820,6 @@ __global__ void __launch_bounds__(NTHR, 1) tdt_decode_kernel(TdtParams p) {
 }
 
 __global__ void tdt_init_kernel(TdtParams p) {
-    pdl_wait();
-    pdl_trigger();
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b < GBAR * GBAR_STRIDE) p.bar[b] = 0u;
     if (b < 3 * p.Bpad) {
@@ -843,8 +840,6 @@ __global__ void boost_state_reset_kernel(DeviceTrie trie, int V, int row0, int n
 
 // fp32 rows [rows][K] -> pre-split rows [rows][2 K] = [hi: K][lo: K] bf16
 __global__ void tdt_split_rows_kernel(const float *__restrict__ src, int rows, int K, bf16 *__restrict__ dst) {
-    pdl_wait();
-    pdl_trigger();
     const size_t n = (size_t)rows * K;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
         const size_t r = i / K;
@@ -928,7 +923,7 @@ cudaError_t launch_cl(TdtParams p, int num_sms, cudaStream_t st, bool *fits, Tdt
             p.out_in_smem = out_in_smem ? 1 : 0;
             p.wih_in_smem = wih_in_smem ? 1 : 0;
             p.smem_lstm_floats = lstm_floats;
-            p.wstage_rows = (getenv("PK_TDT_NO_STAGE") || (ctl && ctl->no_stage)) ? 0 : wstage_rows;
+            p.wstage_rows = (ctl && ctl->no_stage) ? 0 : wstage_rows;
             *fits = true;
             if (ctl) {
                 const TdtGeom ge = tdt_geom(p.P, p.J, p.V + p.D, nc, CL);
@@ -999,7 +994,6 @@ cudaError_t launch_tdt_decode(TdtParams p, int num_sms, cudaStream_t st, TdtLaun
     // The cluster size is decided for every launch from its shapes and the occupancy query: 4 where it fits, else 2.
     int cl = 4;
     if (ctl && ctl->cluster) cl = ctl->cluster;
-    else if (const char *ev = getenv("PK_TDT_CLUSTER")) cl = atoi(ev) == 2 ? 2 : 4;
     const bool fallback = !(ctl && ctl->cluster);
     if (ctl) ctl->grid = 0;
     bool fits = false;

@@ -39,7 +39,7 @@ Coverage (synthetic weights from synth.make_weights; Tmax = 188, above every bat
   tiny                  d 128, 2 heads, hd 64              T = 100 (few-row GEMM)         T = 1, 63, 65, 127, 129
   110m-width, 3 layers  d 512, 8 heads, ff 2048, mel 80    as tiny                        as tiny
   600m-width, 2 layers  d 1024, hd 128, ff 4096, mel 128   as tiny                        as tiny (staged-Q attention)
-Each batch in bf16x3, bf16x1 and fp32; for tiny and 110m-width also PK_GEMM_SKINNY=0 on (a), PK_GEMM_CLUSTER=2 and 4 on (b)
+Each batch in bf16x3, bf16x1 and fp32; for tiny and 110m-width also PK_GEMM_CLUSTER=2 and 4 on (b)
 and PK_ATTN_TC=0 (fp32 attention with a BIAS_F32 QKV) on (b), in bf16x3.  Bitwise engine checks: a stop run twice gives
 the same bytes, the layers tap of layer i equals stop 4 (i + 1), every row of the batch is finite.
 
@@ -293,7 +293,6 @@ def device_states(pkg, e, feats, n_layers, monkeypatch):
 MATH = {"x3": MATH_X3, "x1": MATH_X1, "f32": MATH_F32}
 # (width, variant, math, env, batches)
 RUNS = [(w, m, m, {}, ("a", "b")) for w in WIDTHS for m in MATH]
-RUNS += [(w, "skinny0", "x3", {"PK_GEMM_SKINNY": "0"}, ("a",)) for w in ("tiny", "110m")]
 RUNS += [(w, f"cluster{c}", "x3", {"PK_GEMM_CLUSTER": str(c)}, ("b",)) for w in ("tiny", "110m") for c in (2, 4)]
 RUNS += [(w, "attn_tc0", "x3", {"PK_ATTN_TC": "0"}, ("b",)) for w in ("tiny", "110m")]
 
