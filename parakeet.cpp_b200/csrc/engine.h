@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -76,6 +77,62 @@ static_assert(BOOST_SLOT_NODES == PK_BOOST_ROW_NODES, "the slot capacity is part
 
 }  // namespace pk_detail
 using namespace pk_detail;
+
+// The open streams of an engine (stream_engine.cu): ASR streams (pk_stream_open) or Sortformer streams (pk_diar_stream_open).
+struct StreamSet {
+    int S = 0, L = 70, R = 1, max_chunk = 0;
+    int nf_max = 0, take_max = 0, c_max = 0;
+    // host bookkeeping
+    std::vector<int32_t> ovl_len, left, cache_len, ring_start, frame_base;
+    std::vector<int32_t> act, take, nC;                       // this step: active stream ids, frames taken, encoder frames
+    // device state
+    StreamState st{};
+    float *kc = nullptr, *vc = nullptr;                        // [layers][S][L][d]
+    float *convc = nullptr;                                    // [layers][S][k-1][d]
+    float *c_state = nullptr;                                  // [lstm][Bpad][P]
+    float *hbuf = nullptr;                                     // bf16 planes [hi|lo][lstm][2][Bpad][P]
+    int32_t *tok_state = nullptr;
+    // Phrase boosting per stream (pk_stream_set_boost): a trie slot and score per stream, and the trie state of the decode
+    // kernel, carried from chunk to chunk like the LSTM state.
+    BoostSlots boost;
+    uint32_t *boost_bits = nullptr;                            // [Bpad][(V+31)/32]
+    int32_t *trie_active = nullptr, *trie_nact = nullptr;      // [Bpad][64], [Bpad]
+    std::vector<uint8_t> boosted;                              // stream has a list
+    int n_boosted = 0;
+    // per-step device scratch
+    float *d_chunk = nullptr, *ssig = nullptr, *mel_in = nullptr;
+    StreamPlan *d_plan = nullptr, *h_plan = nullptr;           // h_plan pinned
+    int64_t *d_sig_off = nullptr, *h_sig_off = nullptr;
+    int32_t *d_meta = nullptr, *h_meta = nullptr;              // nf | out_row | act | cache_len | ring_start | frame_base | row_off_S
+    float *h_chunk = nullptr;                                  // pinned staging of the chunk samples
+    cudaEvent_t ev_up = nullptr;                               // uploads of the previous step consumed
+    size_t state_bytes = 0;
+    // Sortformer streams (pk_diar_stream_open): no sample overlap, LSTM or token state; h_meta [0, S] holds the mel frame
+    // offsets of the step's chunks, d_chunk / d_sig_off the packed PCM and its offsets.
+    bool diar = false;
+    float *mel_new = nullptr, *h_mel = nullptr;                // this step's log-mel frames [S * nf_max][mel] (h_mel pinned)
+    std::vector<uint64_t> spk_seen;                            // AOSCCache::speaker_active_ (max_speakers <= 64)
+    std::vector<std::vector<int32_t>> arrival;                 // AOSCCache::arrival_order_
+
+    // After a step that gave stream i the encoder rows [row_off[i], row_off[i+1]): its K / V rings hold the last L rows,
+    // cache_len of them from ring_start on (streaming_encoder.cpp:185-208), which the cached attention reads next step.
+    void advance(const int32_t *row_off) {
+        for (int i = 0; i < S; ++i) {
+            const int C = row_off[i + 1] - row_off[i], kv = cache_len[i] + C;
+            if (kv > L) ring_start[i] = (ring_start[i] + kv - L) % L;
+            cache_len[i] = std::min(kv, L);
+            frame_base[i] += C;
+        }
+    }
+    // CUDA-graph key of a step: every kernel argument depends only on which streams take how many frames.  The tag keeps
+    // the caches of different step kinds apart.
+    std::string graph_key(char tag) const {
+        std::string key(1, tag);
+        key.append(reinterpret_cast<const char *>(act.data()), act.size() * sizeof(int32_t));
+        key.append(reinterpret_cast<const char *>(take.data()), take.size() * sizeof(int32_t));
+        return key;
+    }
+};
 
 struct pk_engine {
     pk_config cfg;
@@ -298,11 +355,10 @@ struct pk_engine {
     pk_status set_batch_shapes(const int32_t *n_frames_or_null, const int64_t *offsets_or_null, int n);
     pk_status upload_shapes();
     void gemm(const Act &A, int lda, const GemmWeight &W, int M_, EpiParams epi);
-    // x = resid + alpha * (A . W^T + b) (the residual GEMM) followed by LayerNorm(s) (layernorm_kernel).  resid_in_x: the
-    // residual is x itself (false: x = A . W^T + b).
-    // out_ln1: x receives LayerNorm_1 of the sum (block end) instead of the sum; planes = split of the last LayerNorm.
-    pk_status gemm_ln(const Act &A, int lda, const GemmWeight &W, int M_, bool resid_in_x, float alpha, const float *ln1_w, const float *ln1_b,
-                      bool out_ln1, const float *ln2_w, const float *ln2_b, ActBuf planes);
+    // LayerNorm of the M rows of `in` [M][width] (layernorm_kernel) into out1 / act1; with w2, a second LayerNorm of that
+    // result into act2.
+    void layernorm(const float *in, int width, const float *w1, const float *b1, float *out1, ActBuf act1, const float *w2 = nullptr,
+                   const float *b2 = nullptr, ActBuf act2 = {});
     int gemm_cluster = 0;                      // PK_GEMM_CLUSTER=2|4: wide GEMMs (fc1, q/k/v, pw1) run as clusters of 2 | 4 CTAs along N with the A tile multicast
     // few-row GEMMs (M <= 128: streaming steps, short utterances) go to gemm_skinny.cu (offline diarization keeps it off)
     bool skinny = true;
@@ -314,19 +370,21 @@ struct pk_engine {
     pk_status run_mel(int u0 = 0, int u1 = -1);
     pk_status run_conv1(int u0 = 0, int u1 = -1);
     pk_status run_graphed(const std::string &key, const std::function<pk_status()> &body);
-    pk_status run_subsample_tail(bool with_first_ln = false);
+    pk_status run_subsample_tail();
     pk_status run_encoder(float *sub_out_host, float *layers_out_host);
+    // The Conformer blocks on the rows in x; cached: a step of the open streams (attention over their K / V rings, causal
+    // conv over their conv caches).  layers_out_host (offline only, may be null) receives x after every block.
+    pk_status run_blocks(bool cached, float *layers_out_host);
     // streaming eou path (stream_engine.cu); on a Sortformer engine the streams of pk_diar_stream_open
-    struct StreamSet *ss = nullptr;
-    pk_status run_stream_layers();
+    StreamSet *ss = nullptr;
     pk_status run_stream_decode();
-    pk_status run_ctc(float *logprobs_dev_or_null);
+    // dec: PK_DECODER_CTC, _CTC_BEAM or _CTC_ALIGN; logprobs_dev_or_null: where the log-probs land (null: where the decoder needs them)
+    pk_status run_ctc(pk_decoder dec, float *logprobs_dev_or_null);
     pk_status run_tdt();
-    pk_status run_ctc_beam();
-    pk_status run_ctc_align();
+    pk_status tdt_decode(TdtParams &p);               // enc_proj and the decode kernel; p holds what the caller's decode sets
     pk_status run_decoder(pk_decoder dec) {           // (dec already checked)
-        if (dec == PK_DECODER_CTC_ALIGN) return run_ctc_align();
-        return dec == PK_DECODER_CTC ? run_ctc(nullptr) : (dec == PK_DECODER_CTC_BEAM ? run_ctc_beam() : run_tdt());
+        const bool ctc = dec == PK_DECODER_CTC || dec == PK_DECODER_CTC_BEAM || dec == PK_DECODER_CTC_ALIGN;
+        return ctc ? run_ctc(dec, nullptr) : run_tdt();
     }
     pk_status fetch(pk_tokens *out);
 };

@@ -137,7 +137,7 @@ pk_status pk_kernel_gemm(int device, int path, int math, int cluster, int M, int
     bf16 *oh = planes ? cx.guarded<bf16>(n_o) : nullptr, *ol = planes && out_lo ? cx.guarded<bf16>(n_o) : nullptr;
     float *dr = nullptr;
     if (resid_k) {
-        if (in_place) {          // out_f32 starts as the residual and aliases it, as in pk_engine::gemm_ln
+        if (in_place) {          // out_f32 starts as the residual and aliases it, as in pk_engine::run_blocks
             if (cudaMemcpy(of, resid, n_o * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) return PK_ERR_CUDA;
             dr = of;
         } else {
@@ -259,7 +259,7 @@ pk_status pk_kernel_layernorm(int device, int M, int d, const float *x, const fl
     float *dw1 = cx.upload(w1, d), *db1 = cx.upload(b1, d), *dw2 = w2 ? cx.upload(w2, d) : nullptr, *db2 = b2 ? cx.upload(b2, d) : nullptr;
     float *y1 = want_f32 ? cx.guarded<float>(n) : nullptr;
     float *dx;
-    if (y1) {                 // LN1 written in place over its input, as pk_engine::gemm_ln does
+    if (y1) {                 // LN1 written in place over its input, as pk_engine::run_blocks does
         if (cudaMemcpy(y1, x, n * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) return PK_ERR_CUDA;
         dx = y1;
     } else {
