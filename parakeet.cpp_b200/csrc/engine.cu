@@ -466,7 +466,7 @@ pk_status pk_engine::set_batch_shapes(const int32_t *n_frames, const int64_t *of
             if (F < 2) return fail(PK_ERR_INVALID, "utterance needs at least 2 mel frames");
             if (F > Fmax) return fail(PK_ERR_CAPACITY, "utterance exceeds max frames");
         }
-        const int t1 = conv_len(F), t2 = conv_len(t1), T = conv_len(t2);
+        const int t2 = conv_len(conv_len(F)), T = enc_frames(F);
         frame_off[i + 1] = frame_off[i] + F;
         s2_off[i + 1] = s2_off[i] + t2;
         row_off[i + 1] = row_off[i] + T;
@@ -605,7 +605,7 @@ pk_status pk_engine::run_blocks(bool cached, float *layers_out_host) {
     const int32_t *s_act = nullptr, *s_cl = nullptr, *s_rs = nullptr;
     int n_act = 0, maxC = 0;
     if (cached) {
-        s_act = ss->d_meta + 2 * ss->S; s_cl = ss->d_meta + 3 * ss->S; s_rs = ss->d_meta + 4 * ss->S;
+        s_act = ss->meta_d(StreamSet::ACT); s_cl = ss->meta_d(StreamSet::CACHE_LEN); s_rs = ss->meta_d(StreamSet::RING_START);
         n_act = (int)ss->act.size();
         for (int n : ss->nC) maxC = std::max(maxC, n);
     }
@@ -981,7 +981,7 @@ void pk_config_nemotron_600m(pk_config *c) {
 }
 
 int32_t pk_mel_frames(int64_t n_samples) { return (int32_t)(1 + n_samples / 160); }
-int32_t pk_encoder_frames(int32_t f) { return conv_len(conv_len(conv_len(f))); }
+int32_t pk_encoder_frames(int32_t f) { return enc_frames(f); }
 
 const char *pk_last_error(const pk_engine *e) { return e ? e->err.c_str() : g_create_err.c_str(); }
 

@@ -35,6 +35,7 @@ std::string &create_err();   // last error of a failed pk_engine_create / engine
     } while (0)
 
 inline int conv_len(int L) { return (L - 1) / 2 + 1; }  // k3 s2 p1 (operations.cpp:3191-3196)
+inline int enc_frames(int mel_frames) { return conv_len(conv_len(conv_len(mel_frames))); }   // the three stride-2 convs
 
 // A linear layer's parameters on the device: fp32 master [N][K] + bias, and (wgmma
 // modes) the bf16 hi/lo split planes of the weight.
@@ -103,16 +104,36 @@ struct StreamSet {
     float *d_chunk = nullptr, *ssig = nullptr, *mel_in = nullptr;
     StreamPlan *d_plan = nullptr, *h_plan = nullptr;           // h_plan pinned
     int64_t *d_sig_off = nullptr, *h_sig_off = nullptr;
-    int32_t *d_meta = nullptr, *h_meta = nullptr;              // nf | out_row | act | cache_len | ring_start | frame_base | row_off_S
+    int32_t *d_meta = nullptr, *h_meta = nullptr;              // the step's metadata (Meta), h_meta pinned
     float *h_chunk = nullptr;                                  // pinned staging of the chunk samples
     cudaEvent_t ev_up = nullptr;                               // uploads of the previous step consumed
     size_t state_bytes = 0;
-    // Sortformer streams (pk_diar_stream_open): no sample overlap, LSTM or token state; h_meta [0, S] holds the mel frame
-    // offsets of the step's chunks, d_chunk / d_sig_off the packed PCM and its offsets.
+    // Sortformer streams (pk_diar_stream_open): no sample overlap, LSTM or token state; d_chunk / d_sig_off hold the packed
+    // PCM and its offsets.
     bool diar = false;
     float *mel_new = nullptr, *h_mel = nullptr;                // this step's log-mel frames [S * nf_max][mel] (h_mel pinned)
     std::vector<uint64_t> spk_seen;                            // AOSCCache::speaker_active_ (max_speakers <= 64)
     std::vector<std::vector<int32_t>> arrival;                 // AOSCCache::arrival_order_
+
+    StreamSet() = default;
+    StreamSet(const StreamSet &) = delete;
+    StreamSet &operator=(const StreamSet &) = delete;
+    ~StreamSet() {                                             // the device buffers belong to the engine (pk_engine::allocs)
+        if (h_plan) cudaFreeHost(h_plan);
+        if (h_sig_off) cudaFreeHost(h_sig_off);
+        if (h_meta) cudaFreeHost(h_meta);
+        if (h_chunk) cudaFreeHost(h_chunk);
+        if (h_mel) cudaFreeHost(h_mel);
+        if (ev_up) cudaEventDestroy(ev_up);
+    }
+
+    // The segments of h_meta / d_meta, S ints each and row_off S + 1: nf | out_row | act | cache_len | ring_start |
+    // frame_base | row_off, meta_ints() uploaded per step.  Sortformer streams keep the mel frame offsets of the step's
+    // chunks (S + 1 ints, mel_off) in place of nf | out_row.
+    enum Meta : int { NF, OUT_ROW, ACT, CACHE_LEN, RING_START, FRAME_BASE, ROW_OFF, MEL_OFF = NF };
+    int32_t *meta_h(Meta k) const { return h_meta + (size_t)k * S; }
+    int32_t *meta_d(Meta k) const { return d_meta + (size_t)k * S; }
+    size_t meta_ints() const { return (size_t)ROW_OFF * S + S + 1; }
 
     // After a step that gave stream i the encoder rows [row_off[i], row_off[i+1]): its K / V rings hold the last L rows,
     // cache_len of them from ring_start on (streaming_encoder.cpp:185-208), which the cached attention reads next step.
@@ -377,7 +398,6 @@ struct pk_engine {
     pk_status run_blocks(bool cached, float *layers_out_host);
     // streaming eou path (stream_engine.cu); on a Sortformer engine the streams of pk_diar_stream_open
     StreamSet *ss = nullptr;
-    pk_status run_stream_decode();
     // dec: PK_DECODER_CTC, _CTC_BEAM or _CTC_ALIGN; logprobs_dev_or_null: where the log-probs land (null: where the decoder needs them)
     pk_status run_ctc(pk_decoder dec, float *logprobs_dev_or_null);
     pk_status run_tdt();
