@@ -52,6 +52,11 @@ struct EncoderConfig {
     int mel_bins = 80, subsampling_factor = 8, subsampling_channels = 256, hidden_size = 1024, num_layers = 24,
         num_heads = 8, ffn_intermediate = 4096, conv_kernel_size = 9;
     float dropout = 0.1f, layer_norm_eps = 1e-5f;
+    // Limited-context attention for long offline utterances (pk_config.local_att_left / _right; 0, 0 = full attention).
+    // With a band, max_samples may go up to PK_LOCAL_ATT_MAX_SAMPLES / max_batch (3 h for one utterance):
+    //     auto cfg = make_110m_config(); cfg.encoder.local_att_left = cfg.encoder.local_att_right = 256;
+    //     Transcriber t(w, vocab, cfg, 0, /*max_batch=*/1, /*max_samples=*/3600 * 16000);
+    int local_att_left = 0, local_att_right = 0;
 };
 struct PredictionConfig { int vocab_size = 1025, pred_hidden = 640, num_lstm_layers = 2; float dropout = 0.1f; };
 struct JointConfig { int encoder_hidden = 1024, pred_hidden = 640, joint_hidden = 640, vocab_size = 1025; };
@@ -352,6 +357,7 @@ class EngineHolder {
 inline void fill(pk_config &c, const EncoderConfig &e, const PredictionConfig &p, const JointConfig &j, const std::vector<int> &dur) {
     c.mel_bins = e.mel_bins; c.sub_channels = e.subsampling_channels; c.d_model = e.hidden_size; c.n_layers = e.num_layers;
     c.n_heads = e.num_heads; c.ff = e.ffn_intermediate; c.conv_kernel = e.conv_kernel_size;
+    c.local_att_left = e.local_att_left; c.local_att_right = e.local_att_right;
     c.vocab = j.vocab_size; c.pred_hidden = p.pred_hidden; c.lstm_layers = p.num_lstm_layers; c.joint_hidden = j.joint_hidden;
     c.n_durations = (int)dur.size();
     for (size_t i = 0; i < dur.size() && i < 8; ++i) c.durations[i] = dur[i];

@@ -74,9 +74,22 @@ typedef struct {
                                   advances a frame after this many emissions on it */
     /* engine capacity (not model shape) */
     int32_t max_batch;         /* utterances per call */
-    int32_t max_samples;       /* per utterance */
+    int32_t max_samples;       /* per utterance; with full attention the position tables and the attention grow with
+                                  the square of it, with a band (below) linearly */
     int32_t math;              /* pk_math */
+    /* Limited-context attention (NeMo's rel_pos_local_attn, DESIGN.md section 16) for long offline utterances: encoder
+     * frame i attends to frame j only when -local_att_right <= i - j <= local_att_left, with the same relative-position
+     * bias and the softmax over the keys that remain.  Both >= 0 (PK_ERR_INVALID otherwise); 0, 0 = full attention, the
+     * default of every preset.  A band engine keeps position tables of 2 min(max(left, right), T'max - 1) + 1 rows (T'max =
+     * the encoder frames of max_samples: a band wider than an utterance is full attention, at its cost).  It supports
+     * max_samples <= PK_LOCAL_ATT_MAX_SAMPLES (3 h of 16 kHz audio; pk_engine_create returns PK_ERR_CAPACITY past it) and
+     * batches of at most the encoder frames of that much audio in all (PK_ERR_CAPACITY from the call otherwise).
+     * It runs every offline entry point; pk_stream_open on it is PK_ERR_INVALID, and a Sortformer engine takes no band. */
+    int32_t local_att_left;
+    int32_t local_att_right;
 } pk_config;
+
+#define PK_LOCAL_ATT_MAX_SAMPLES 172800000
 
 typedef struct pk_engine pk_engine;
 
@@ -280,6 +293,12 @@ pk_status pk_kernel_gemm(int device, int path, int math, int cluster, int M, int
 pk_status pk_kernel_attention(int device, int kernel, int math, int n_utt, const int32_t *row_off, int rows_total, int d_model, int n_heads,
                               int tmax, const float *qkv, const float *pp, const float *pos_u, const float *pos_v, float *ctx_f32,
                               float *ctx_hi, float *ctx_lo, int64_t *guard_bad);
+/* The same with a band (left, right), both >= 0 and not both 0, as a band engine runs it: pp [2 tmax - 1][d] holds the
+ * relative positions -(tmax-1)..tmax-1, tmax >= max(left, right) + 1 (the engine's table: tmax = max(left, right) + 1 when
+ * that is below its T'max); utterances may be longer than tmax.  The table is uploaded between two NaN rows, which the kernel must not read. */
+pk_status pk_kernel_attention_local(int device, int kernel, int math, int n_utt, const int32_t *row_off, int rows_total, int d_model,
+                                    int n_heads, int tmax, int left, int right, const float *qkv, const float *pp, const float *pos_u,
+                                    const float *pos_v, float *ctx_f32, float *ctx_hi, float *ctx_lo, int64_t *guard_bad);
 /* LayerNorm of x [M][d] (w2 == NULL: one; else LN2(LN1(x)), the chained form).  want_f32: y1 = LN1(x) written in place over
  * x -> y1_f32.  planes (the operand of the last LayerNorm): 0 none, 1 hi, 2 hi + lo, 3 fp32 -> act_f32. */
 pk_status pk_kernel_layernorm(int device, int M, int d, const float *x, const float *w1, const float *b1, const float *w2, const float *b2,

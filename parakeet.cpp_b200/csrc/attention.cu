@@ -13,6 +13,13 @@
 // materialised.  No mask: Transcriber never passes one (transcribe.hpp:108); keys beyond
 // the utterance's own length are excluded, which is what batch=1 in the reference means.
 //
+// Limited context (rel_pos_local_attn, DESIGN.md section 16): with a band (left, right) query i
+// attends to key j only when -right <= i - j <= left; the softmax runs over the keys that remain.
+// A query tile visits only the key tiles that meet [i0 - left, i0 + BQ - 1 + right], starting on
+// multiples of BKV, and masks per element inside them.  The table then needs only the relative
+// positions -W..W (W = max(left, right), tmax = W + 1); window rows outside it are zero-filled and
+// every score that would read them is masked.  The launchers map the band (0, 0) to full attention.
+//
 // fp32 CUDA-core flash-style kernel: one CTA per (query tile, head, utterance); key tiles
 // stream through shared memory with an online softmax; 4x4 register blocking; operands
 // are stored transposed ([k][row]) so the inner loop uses float4 shared loads.
@@ -35,7 +42,7 @@ template <int HD, int BQ, int BKV>
 __global__ void __launch_bounds__(AttnCfg<HD, BQ, BKV>::THREADS)
 relpos_attention_kernel(const float *__restrict__ qkv, int ld_qkv, const int32_t *__restrict__ row_off,
                         const float *__restrict__ pp, int tmax, const float *__restrict__ bias_u,
-                        const float *__restrict__ bias_v, int d_model, ActBuf out) {
+                        const float *__restrict__ bias_v, int left, int right, int d_model, ActBuf out) {
     using C = AttnCfg<HD, BQ, BKV>;
     extern __shared__ __align__(16) float sm[];
     float *Qu_t = sm;                      // [HD][LQ]
@@ -70,7 +77,8 @@ relpos_attention_kernel(const float *__restrict__ qkv, int ld_qkv, const int32_t
         for (int c = 0; c < C::CPT; ++c) o[a][c] = 0.f;
     }
 
-    for (int j0 = 0; j0 < T; j0 += BKV) {
+    const int j_lo = max(i0 - left, 0) / BKV * BKV, j_hi = min(T, i0 + BQ + right);
+    for (int j0 = j_lo; j0 < j_hi; j0 += BKV) {
         __syncthreads();  // previous tile fully consumed (also orders the Q stores on first pass)
         // ---- K (transposed), V (natural), PP window (transposed)
         for (int idx = tid; idx < BKV * HD; idx += C::THREADS) {
@@ -128,7 +136,8 @@ relpos_attention_kernel(const float *__restrict__ qkv, int ld_qkv, const int32_t
             float mx = -INFINITY;
 #pragma unroll
             for (int bb = 0; bb < 4; ++bb) {
-                const bool valid = (j0 + tx * 4 + bb) < T;
+                const int j = j0 + tx * 4 + bb, dij = i0 + ty * 4 + a - j;
+                const bool valid = j < T && dij <= left && -dij <= right;
                 s[a][bb] = valid ? s[a][bb] * scale : -INFINITY;
                 mx = fmaxf(mx, s[a][bb]);
             }
@@ -191,7 +200,7 @@ relpos_attention_kernel(const float *__restrict__ qkv, int ld_qkv, const int32_t
 
 template <int HD, int BQ, int BKV>
 void launch_t(const float *qkv, int ld_qkv, const int32_t *row_off, int n_utt, int max_T, int n_heads,
-              const float *pp, int tmax, const float *bu, const float *bv, int d_model, ActBuf out,
+              const float *pp, int tmax, const float *bu, const float *bv, int left, int right, int d_model, ActBuf out,
               cudaStream_t st) {
     using C = AttnCfg<HD, BQ, BKV>;
     static PerDeviceFlag attr_flag;
@@ -203,18 +212,20 @@ void launch_t(const float *qkv, int ld_qkv, const int32_t *row_off, int n_utt, i
     }
     dim3 grid((max_T + BQ - 1) / BQ, n_heads, n_utt);
     relpos_attention_kernel<HD, BQ, BKV><<<dim3(grid), dim3(C::THREADS), C::SMEM, st>>>(qkv, ld_qkv, row_off, pp, tmax, bu,
-                                                                           bv, d_model, out);
+                                                                           bv, left, right, d_model, out);
 }
 
 }  // namespace
 
 bool launch_relpos_attention(const float *qkv, int ld_qkv, const int32_t *row_off, int n_utt, int max_T,
-                             int n_heads, int head_dim, const float *pp, int tmax, const float *bu,
-                             const float *bv, int d_model, ActBuf out, cudaStream_t st) {
+                             int n_heads, int head_dim, const float *pp, int tmax, int att_left, int att_right,
+                             const float *bu, const float *bv, int d_model, ActBuf out, cudaStream_t st) {
+    int left, right;
+    if (!attention_band(att_left, att_right, &left, &right)) return false;
     if (head_dim == 64) {
-        launch_t<64, 64, 64>(qkv, ld_qkv, row_off, n_utt, max_T, n_heads, pp, tmax, bu, bv, d_model, out, st);
+        launch_t<64, 64, 64>(qkv, ld_qkv, row_off, n_utt, max_T, n_heads, pp, tmax, bu, bv, left, right, d_model, out, st);
     } else if (head_dim == 128) {
-        launch_t<128, 64, 32>(qkv, ld_qkv, row_off, n_utt, max_T, n_heads, pp, tmax, bu, bv, d_model, out, st);
+        launch_t<128, 64, 32>(qkv, ld_qkv, row_off, n_utt, max_T, n_heads, pp, tmax, bu, bv, left, right, d_model, out, st);
     } else {
         return false;
     }

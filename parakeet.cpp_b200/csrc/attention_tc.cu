@@ -101,7 +101,7 @@ __global__ void __launch_bounds__(TCA_THREADS, QS ? 1 : 2)
 relpos_attention_tc_kernel(const float *__restrict__ q32, const float *__restrict__ pos_u, const float *__restrict__ pos_v,
                            const bf16 *__restrict__ qkv_hi, const bf16 *__restrict__ qkv_lo, int ld_qkv,
                            const int32_t *__restrict__ row_off, const bf16 *__restrict__ pp_hi,
-                           const bf16 *__restrict__ pp_lo, int tmax, int d_model, ActBuf out) {
+                           const bf16 *__restrict__ pp_lo, int tmax, int left, int right, int d_model, ActBuf out) {
     extern __shared__ __align__(16) uint8_t smraw[];
     using SM = AttnSmem<HD, QS>;
     constexpr int LDS_ = SM::LDS_, KS = HD / 16, NBO = HD / 8, CH = HD / 8;   // k-steps, output n-blocks, 16 B chunks per row
@@ -150,7 +150,10 @@ relpos_attention_tc_kernel(const float *__restrict__ q32, const float *__restric
     const uint32_t sk_hi = smem_addr(sm.k_hi), sk_lo = smem_addr(sm.k_lo), sv_hi = smem_addr(sm.v_hi), sv_lo = smem_addr(sm.v_lo);
     const uint32_t sp_hi = smem_addr(sm.pp_hi), sp_lo = smem_addr(sm.pp_lo);
 
-    for (int j0 = 0; j0 < T; j0 += BKV) {
+    // key tiles that meet [i0 - left, i0 + BQ - 1 + right] n [0, T), starting on multiples of BKV: a band that covers the
+    // utterance visits the same tiles in the same order as full attention
+    const int j_lo = max(i0 - left, 0) / BKV * BKV, j_hi = min(T, i0 + BQ + right);
+    for (int j0 = j_lo; j0 < j_hi; j0 += BKV) {
         __syncthreads();                 // previous key tile fully consumed
         // ---- K, V rows j0..j0+63 and the PP window, 16 B per cp.async
         for (int idx = tid; idx < BKV * CH; idx += TCA_THREADS) {
@@ -176,7 +179,7 @@ relpos_attention_tc_kernel(const float *__restrict__ q32, const float *__restric
             cp_async16(sp_lo + so, pp_lo + o, nb);
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
-        if (!QS && j0 == 0) {
+        if (!QS && j0 == j_lo) {
             // Q fragments: Qu = q + pos_bias_u, Qv = q + pos_bias_v, split hi/lo (rows past T stay zero)
             const int ia = i0 + wrow + g, ib = ia + 8;
 #pragma unroll
@@ -195,7 +198,7 @@ relpos_attention_tc_kernel(const float *__restrict__ q32, const float *__restric
                     }
                 }
         }
-        if (QS && j0 == 0) {
+        if (QS && j0 == j_lo) {
             // Qu / Qv tiles (hi, lo) -> shared memory while the first key tile is on its way; visible after the barrier below
 #pragma unroll
             for (int it = 0; it < NQ; ++it) {
@@ -300,27 +303,31 @@ relpos_attention_tc_kernel(const float *__restrict__ q32, const float *__restric
         float alpha[2];
 #pragma unroll
         for (int hrow = 0; hrow < 2; ++hrow) {
+            const int i = i0 + wrow + g + hrow * 8;
             float mx = -INFINITY;
 #pragma unroll
             for (int nb = 0; nb < 8; ++nb)
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                    const int jj = nb * 8 + 2 * c + e;
+                    const int jj = nb * 8 + 2 * c + e, dij = i - (j0 + jj);
                     float s = sacc[nb][hrow * 2 + e] * kScale;
-                    s = (j0 + jj < T) ? s : -INFINITY;
+                    s = (j0 + jj < T && dij <= left && -dij <= right) ? s : -INFINITY;
                     sacc[nb][hrow * 2 + e] = s;
                     mx = fmaxf(mx, s);
                 }
             mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
             mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-            const float m_new = fmaxf(m_run[hrow], mx);     // finite: key j0 is always valid
-            alpha[hrow] = ex2_approx(m_run[hrow] - m_new);  // ex2(-inf) = 0 on the first tile
+            // Full attention: finite from the first tile on (key j0 is valid).  A band can mask every key a row has seen so
+            // far; such a row keeps m = -inf and is shifted by 0 instead: p = ex2(-inf) = 0 and alpha scales l = 0, O = 0.
+            const float m_new = fmaxf(m_run[hrow], mx);
+            const float m_sh = m_new == -INFINITY ? 0.f : m_new;
+            alpha[hrow] = ex2_approx(m_run[hrow] - m_sh);   // ex2(-inf) = 0 on the first tile
             float sum = 0.f;
 #pragma unroll
             for (int nb = 0; nb < 8; ++nb)
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                    const float pexp = ex2_approx(sacc[nb][hrow * 2 + e] - m_new);
+                    const float pexp = ex2_approx(sacc[nb][hrow * 2 + e] - m_sh);
                     sacc[nb][hrow * 2 + e] = pexp;
                     sum += pexp;
                 }
@@ -384,7 +391,8 @@ relpos_attention_tc_kernel(const float *__restrict__ q32, const float *__restric
 template <int HD, bool QS>
 static bool launch_attn_t(const float *q32, const float *pos_u, const float *pos_v, const bf16 *qkv_hi, const bf16 *qkv_lo, int ld_qkv,
                           const int32_t *row_off, int n_utt, int max_T,
-                          int n_heads, const bf16 *pp_hi, const bf16 *pp_lo, int tmax, int d_model, ActBuf out, cudaStream_t st) {
+                          int n_heads, const bf16 *pp_hi, const bf16 *pp_lo, int tmax, int left, int right, int d_model, ActBuf out,
+                          cudaStream_t st) {
     using SM = AttnSmem<HD, QS>;
     static PerDeviceFlag attr_flag;
     bool &attr = attr_flag.cur();
@@ -396,18 +404,22 @@ static bool launch_attn_t(const float *q32, const float *pos_u, const float *pos
     }
     dim3 grid((max_T + BQ - 1) / BQ, n_heads, n_utt);
     relpos_attention_tc_kernel<HD, QS><<<dim3(grid), dim3(TCA_THREADS), sizeof(SM), st>>>(q32, pos_u, pos_v, qkv_hi, qkv_lo, ld_qkv, row_off, pp_hi, pp_lo,
-                                                                              tmax, d_model, out);
+                                                                              tmax, left, right, d_model, out);
     return true;
 }
 
 bool launch_relpos_attention_tc(const float *q32, const float *pos_u, const float *pos_v, const bf16 *qkv_hi, const bf16 *qkv_lo,
                                 int ld_qkv, const int32_t *row_off, int n_utt, int max_T, int n_heads, int head_dim, const bf16 *pp_hi,
-                                const bf16 *pp_lo, int tmax, int d_model, ActBuf out, cudaStream_t st) {
+                                const bf16 *pp_lo, int tmax, int att_left, int att_right, int d_model, ActBuf out, cudaStream_t st) {
     if (!q32 || !pos_u || !pos_v || !qkv_hi || !qkv_lo || !pp_hi || !pp_lo) return false;
+    int left, right;
+    if (!attention_band(att_left, att_right, &left, &right)) return false;
     if (head_dim == 64)
-        return launch_attn_t<64, false>(q32, pos_u, pos_v, qkv_hi, qkv_lo, ld_qkv, row_off, n_utt, max_T, n_heads, pp_hi, pp_lo, tmax, d_model, out, st);
+        return launch_attn_t<64, false>(q32, pos_u, pos_v, qkv_hi, qkv_lo, ld_qkv, row_off, n_utt, max_T, n_heads, pp_hi, pp_lo, tmax, left, right,
+                                        d_model, out, st);
     if (head_dim == 128)
-        return launch_attn_t<128, true>(q32, pos_u, pos_v, qkv_hi, qkv_lo, ld_qkv, row_off, n_utt, max_T, n_heads, pp_hi, pp_lo, tmax, d_model, out, st);
+        return launch_attn_t<128, true>(q32, pos_u, pos_v, qkv_hi, qkv_lo, ld_qkv, row_off, n_utt, max_T, n_heads, pp_hi, pp_lo, tmax, left, right,
+                                        d_model, out, st);
     return false;
 }
 

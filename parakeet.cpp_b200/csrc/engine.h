@@ -59,7 +59,7 @@ struct LayerW {
     float *att_ln_w, *att_ln_b;
     GemmWeight qkv, out;
     float *pos_u, *pos_v;
-    float *pp;  // [(2*Tmax-1)][d] projected relative-position table
+    float *pp;  // [(2*pos_tmax-1)][d] projected relative-position table
     bf16 *pp_hi = nullptr, *pp_lo = nullptr;   // its bf16 split planes (tensor-core attention)
     float *conv_ln_w, *conv_ln_b;
     GemmWeight pw1, pw2;
@@ -190,6 +190,8 @@ struct pk_engine {
 
     // ---- capacity
     int Bmax = 0, Fmax = 0, Tmax = 0;          // per-utterance max mel frames / encoder frames
+    int pos_tmax = 0;                          // position tables cover -(pos_tmax-1)..pos_tmax-1: Tmax, or W + 1 for a band
+                                               // (cfg.local_att_left / _right, W = the larger of the two)
     int f1n = 0, f2n = 0, f3n = 0;
     int cap = 0;                               // token capacity per utterance
 
@@ -373,6 +375,7 @@ struct pk_engine {
     pk_status finish_weight(std::vector<float> &w, std::vector<float> *b, int N, int K, GemmWeight &out);
     pk_status get_vec(const SafeTensors &st, const std::string &name, int n, float **out);
     pk_status alloc_workspace();
+    pk_status band_rows_ok();
     pk_status set_batch_shapes(const int32_t *n_frames_or_null, const int64_t *offsets_or_null, int n);
     pk_status upload_shapes();
     void gemm(const Act &A, int lda, const GemmWeight &W, int M_, EpiParams epi);

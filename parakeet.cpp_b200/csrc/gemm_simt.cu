@@ -22,7 +22,7 @@ gemm_simt_kernel(const float *__restrict__ A, int lda, const float *__restrict__
     __shared__ __align__(16) float As[2][BK][BM + 4];
     __shared__ __align__(16) float Bs[2][BK][BN + 4];
     const int tid = threadIdx.x;
-    const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
+    const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;     // row tiles on x: M may exceed 65535 tiles (long front ends)
     const int tx = tid & 15, ty = tid >> 4;
     // loader mapping: 512 float4 per operand tile, 2 per thread: row = idx / 4, kq = idx % 4
     float4 ra[2], rb[2];
@@ -98,7 +98,7 @@ gemm_simt_kernel(const float *__restrict__ A, int lda, const float *__restrict__
 void launch_gemm_simt(const float *A, int lda, const float *W, int ldw, int M, int N, int K,
                       const EpiParams &epi, cudaStream_t st) {
     if (M <= 0 || N <= 0) return;
-    dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
+    dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN);
     gemm_simt_kernel<<<dim3(grid), dim3(256), 0, st>>>(A, lda, W, ldw, M, N, K, epi);
 }
 

@@ -108,6 +108,73 @@ bool offsets_ok(const int32_t *row_off, int n_utt, int rows_total) {
 
 bool is_act_kind(int k) { return k == EPI_BIAS_RELU_ACT || k == EPI_BIAS_SILU_ACT || k == EPI_BIAS_ACT; }
 
+// pk_kernel_attention (band 0, 0: full attention, the table covers every utterance) and pk_kernel_attention_local (a band:
+// the table covers -W..W, W = max(left, right), and sits between two NaN rows)
+pk_status attention_hook(int device, int kernel, int math, int n_utt, const int32_t *row_off, int rows_total, int d_model, int n_heads,
+                         int tmax, int left, int right, const float *qkv, const float *pp, const float *pos_u, const float *pos_v,
+                         float *ctx_f32, float *ctx_hi, float *ctx_lo, int64_t *guard_bad) {
+    if (kernel < 0 || kernel > 1 || !offsets_ok(row_off, n_utt, rows_total) || n_heads < 1 || d_model % n_heads || tmax < 1 || !qkv || !pp ||
+        !pos_u || !pos_v || left < 0 || right < 0)
+        return PK_ERR_INVALID;
+    const bool band = left > 0 || right > 0;
+    const int hd = d_model / n_heads, maxT = max_len(row_off, n_utt);
+    if (maxT < 1 || (band ? std::max(left, right) >= tmax : maxT > tmax)) return PK_ERR_INVALID;
+    // the output is what the engine's ctx buffer holds in that math mode: fp32, or bf16 hi (| lo) planes
+    const bool f32 = math == PK_MATH_FP32;
+    if (f32 ? (kernel != 0 || !ctx_f32) : (!ctx_hi || (math == PK_MATH_BF16X3) != (ctx_lo != nullptr))) return PK_ERR_INVALID;
+    HookCtx cx(device);
+    if (!cx.ok) return PK_ERR_CUDA;
+    const int d = d_model, NP = 2 * tmax - 1;
+    const size_t n_o = (size_t)rows_total * d;
+    int32_t *doff = cx.upload(row_off, n_utt + 1);
+    float *dqkv = cx.upload(qkv, (size_t)rows_total * 3 * d), *dpp;
+    if (band) {              // [NaN row | table | NaN row]
+        std::vector<float> h((size_t)(NP + 2) * d, NAN);
+        memcpy(&h[d], pp, (size_t)NP * d * sizeof(float));
+        dpp = cx.upload(h.data(), h.size());
+        if (dpp) dpp += d;
+    } else {
+        dpp = cx.upload(pp, (size_t)NP * d);
+    }
+    float *du = cx.upload(pos_u, d), *dv = cx.upload(pos_v, d);
+    ActBuf out;
+    out.f32 = f32 ? cx.guarded<float>(n_o) : nullptr;
+    out.hi = f32 ? nullptr : cx.guarded<bf16>(n_o);
+    out.lo = ctx_lo ? cx.guarded<bf16>(n_o) : nullptr;
+    if (!cx.ok) return PK_ERR_CUDA;
+    bool launched;
+    if (kernel == 0) {
+        launched = launch_relpos_attention(dqkv, 3 * d, doff, n_utt, maxT, n_heads, hd, dpp, tmax, left, right, du, dv, d, out, cx.st);
+    } else {
+        // the EPI_QKV_ACT epilogue's layout: q fp32 [M, d], k | v bf16 planes [M, 2 d]; the position table split once at load
+        std::vector<float> hq((size_t)rows_total * d), hkv((size_t)rows_total * 2 * d);
+        for (int r = 0; r < rows_total; ++r) {
+            memcpy(&hq[(size_t)r * d], qkv + (size_t)r * 3 * d, (size_t)d * 4);
+            memcpy(&hkv[(size_t)r * 2 * d], qkv + (size_t)r * 3 * d + d, (size_t)2 * d * 4);
+        }
+        float *dq32 = cx.upload(hq.data(), hq.size()), *dkv = cx.upload(hkv.data(), hkv.size());
+        bf16 *kvh = static_cast<bf16 *>(cx.alloc(hkv.size() * 2)), *kvl = static_cast<bf16 *>(cx.alloc(hkv.size() * 2));
+        // the planes keep the NaN rows around a band's table (the split of NaN is NaN)
+        const int pad = band ? 1 : 0;
+        const size_t np_all = (size_t)(NP + 2 * pad) * d;
+        bf16 *pph = static_cast<bf16 *>(cx.alloc(np_all * 2)), *ppl = static_cast<bf16 *>(cx.alloc(np_all * 2));
+        if (!cx.ok) return PK_ERR_CUDA;
+        ActBuf skv; skv.hi = kvh; skv.lo = kvl;
+        ActBuf spp; spp.hi = pph; spp.lo = ppl;
+        launch_split(dkv, hkv.size(), skv, cx.st);
+        launch_split(dpp - (size_t)pad * d, np_all, spp, cx.st);
+        launched = launch_relpos_attention_tc(dq32, du, dv, kvh, kvl, 2 * d, doff, n_utt, maxT, n_heads, hd, pph + (size_t)pad * d,
+                                              ppl + (size_t)pad * d, tmax, left, right, d, out, cx.st);
+    }
+    if (!launched) return PK_ERR_INVALID;
+    pk_status rc = cx.finish(guard_bad);
+    if (rc) return rc;
+    if (out.f32 && !fetch_f32(ctx_f32, out.f32, n_o)) return PK_ERR_CUDA;
+    if (out.hi && !fetch_bf16(ctx_hi, out.hi, n_o)) return PK_ERR_CUDA;
+    if (out.lo && !fetch_bf16(ctx_lo, out.lo, n_o)) return PK_ERR_CUDA;
+    return PK_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -199,53 +266,16 @@ pk_status pk_kernel_gemm(int device, int path, int math, int cluster, int M, int
 pk_status pk_kernel_attention(int device, int kernel, int math, int n_utt, const int32_t *row_off, int rows_total, int d_model, int n_heads,
                               int tmax, const float *qkv, const float *pp, const float *pos_u, const float *pos_v, float *ctx_f32,
                               float *ctx_hi, float *ctx_lo, int64_t *guard_bad) {
-    if (kernel < 0 || kernel > 1 || !offsets_ok(row_off, n_utt, rows_total) || n_heads < 1 || d_model % n_heads || tmax < 1 || !qkv || !pp ||
-        !pos_u || !pos_v)
-        return PK_ERR_INVALID;
-    const int hd = d_model / n_heads, maxT = max_len(row_off, n_utt);
-    if (maxT > tmax || maxT < 1) return PK_ERR_INVALID;
-    // the output is what the engine's ctx buffer holds in that math mode: fp32, or bf16 hi (| lo) planes
-    const bool f32 = math == PK_MATH_FP32;
-    if (f32 ? (kernel != 0 || !ctx_f32) : (!ctx_hi || (math == PK_MATH_BF16X3) != (ctx_lo != nullptr))) return PK_ERR_INVALID;
-    HookCtx cx(device);
-    if (!cx.ok) return PK_ERR_CUDA;
-    const int d = d_model, NP = 2 * tmax - 1;
-    const size_t n_o = (size_t)rows_total * d;
-    int32_t *doff = cx.upload(row_off, n_utt + 1);
-    float *dqkv = cx.upload(qkv, (size_t)rows_total * 3 * d), *dpp = cx.upload(pp, (size_t)NP * d);
-    float *du = cx.upload(pos_u, d), *dv = cx.upload(pos_v, d);
-    ActBuf out;
-    out.f32 = f32 ? cx.guarded<float>(n_o) : nullptr;
-    out.hi = f32 ? nullptr : cx.guarded<bf16>(n_o);
-    out.lo = ctx_lo ? cx.guarded<bf16>(n_o) : nullptr;
-    if (!cx.ok) return PK_ERR_CUDA;
-    bool launched;
-    if (kernel == 0) {
-        launched = launch_relpos_attention(dqkv, 3 * d, doff, n_utt, maxT, n_heads, hd, dpp, tmax, du, dv, d, out, cx.st);
-    } else {
-        // the EPI_QKV_ACT epilogue's layout: q fp32 [M, d], k | v bf16 planes [M, 2 d]; the position table split once at load
-        std::vector<float> hq((size_t)rows_total * d), hkv((size_t)rows_total * 2 * d);
-        for (int r = 0; r < rows_total; ++r) {
-            memcpy(&hq[(size_t)r * d], qkv + (size_t)r * 3 * d, (size_t)d * 4);
-            memcpy(&hkv[(size_t)r * 2 * d], qkv + (size_t)r * 3 * d + d, (size_t)2 * d * 4);
-        }
-        float *dq32 = cx.upload(hq.data(), hq.size()), *dkv = cx.upload(hkv.data(), hkv.size());
-        bf16 *kvh = static_cast<bf16 *>(cx.alloc(hkv.size() * 2)), *kvl = static_cast<bf16 *>(cx.alloc(hkv.size() * 2));
-        bf16 *pph = static_cast<bf16 *>(cx.alloc((size_t)NP * d * 2)), *ppl = static_cast<bf16 *>(cx.alloc((size_t)NP * d * 2));
-        if (!cx.ok) return PK_ERR_CUDA;
-        ActBuf skv; skv.hi = kvh; skv.lo = kvl;
-        ActBuf spp; spp.hi = pph; spp.lo = ppl;
-        launch_split(dkv, hkv.size(), skv, cx.st);
-        launch_split(dpp, (size_t)NP * d, spp, cx.st);
-        launched = launch_relpos_attention_tc(dq32, du, dv, kvh, kvl, 2 * d, doff, n_utt, maxT, n_heads, hd, pph, ppl, tmax, d, out, cx.st);
-    }
-    if (!launched) return PK_ERR_INVALID;
-    pk_status rc = cx.finish(guard_bad);
-    if (rc) return rc;
-    if (out.f32 && !fetch_f32(ctx_f32, out.f32, n_o)) return PK_ERR_CUDA;
-    if (out.hi && !fetch_bf16(ctx_hi, out.hi, n_o)) return PK_ERR_CUDA;
-    if (out.lo && !fetch_bf16(ctx_lo, out.lo, n_o)) return PK_ERR_CUDA;
-    return PK_OK;
+    return attention_hook(device, kernel, math, n_utt, row_off, rows_total, d_model, n_heads, tmax, 0, 0, qkv, pp, pos_u, pos_v, ctx_f32,
+                          ctx_hi, ctx_lo, guard_bad);
+}
+
+pk_status pk_kernel_attention_local(int device, int kernel, int math, int n_utt, const int32_t *row_off, int rows_total, int d_model,
+                                    int n_heads, int tmax, int left, int right, const float *qkv, const float *pp, const float *pos_u,
+                                    const float *pos_v, float *ctx_f32, float *ctx_hi, float *ctx_lo, int64_t *guard_bad) {
+    if (left < 0 || right < 0 || (left == 0 && right == 0)) return PK_ERR_INVALID;
+    return attention_hook(device, kernel, math, n_utt, row_off, rows_total, d_model, n_heads, tmax, left, right, qkv, pp, pos_u, pos_v,
+                          ctx_f32, ctx_hi, ctx_lo, guard_bad);
 }
 
 pk_status pk_kernel_layernorm(int device, int M, int d, const float *x, const float *w1, const float *b1, const float *w2, const float *b2,

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda.h>
 
+#include <algorithm>
 #include <functional>
 #include <string>
 #include <vector>
@@ -123,16 +124,27 @@ bool launch_dwconv_bn_silu(const float *g, const int32_t *row_off, int n_utt, in
                            const float *w, const float *bias, ActBuf out, cudaStream_t st);
 
 // ------------------------------------------------------------------ attention.cu (K7)
+// Both relative-position attention launchers take a band (att_left, att_right), both >= 0: query i attends to key j only
+// when -att_right <= i - j <= att_left.  (0, 0) is full attention.  pp holds the relative positions -(tmax-1)..tmax-1; a
+// band needs tmax >= max(att_left, att_right) + 1.  A negative band: false.
+inline bool attention_band(int att_left, int att_right, int *left, int *right) {
+    if (att_left < 0 || att_right < 0) return false;
+    constexpr int kFull = 1 << 30;          // wider than any utterance, small enough that i0 + BQ + kFull stays an int
+    const bool full = att_left == 0 && att_right == 0;
+    *left = full ? kFull : std::min(att_left, kFull);
+    *right = full ? kFull : std::min(att_right, kFull);
+    return true;
+}
 bool launch_relpos_attention(const float *qkv, int ld_qkv, const int32_t *row_off, int n_utt, int max_T,
-                             int n_heads, int head_dim, const float *pp, int tmax, const float *bu,
-                             const float *bv, int d_model, ActBuf out, cudaStream_t st);
+                             int n_heads, int head_dim, const float *pp, int tmax, int att_left, int att_right,
+                             const float *bu, const float *bv, int d_model, ActBuf out, cudaStream_t st);
 
 // tensor-core variant (attention_tc.cu, head_dim 64): pp as bf16 hi/lo planes
 // From the EPI_QKV_ACT GEMM epilogue: q32 = fp32 q [M, d] (the kernel adds pos_u / pos_v), kv_hi / kv_lo = bf16 planes
 // [M, ld_kv = 2 d] = [k | v].
 bool launch_relpos_attention_tc(const float *q32, const float *pos_u, const float *pos_v, const bf16 *kv_hi, const bf16 *kv_lo,
                                 int ld_kv, const int32_t *row_off, int n_utt, int max_T, int n_heads, int head_dim, const bf16 *pp_hi,
-                                const bf16 *pp_lo, int tmax, int d_model, ActBuf out, cudaStream_t st);
+                                const bf16 *pp_lo, int tmax, int att_left, int att_right, int d_model, ActBuf out, cudaStream_t st);
 
 // ------------------------------------------------------------------ attention_mha.cu / speaker_head.cu (Sortformer)
 // Plain multi-head attention (transformer.cpp:15-50) over packed utterances, head_dim 24 only (false otherwise): qkv fp32

@@ -172,6 +172,8 @@ pk_status pk_stream_open(pk_engine *e, int32_t n_streams, int32_t max_chunk_samp
     if (e->diar) return e->fail(PK_ERR_INVALID, "pk_stream_open: a Sortformer engine opens its streams with pk_diar_stream_open");
     const pk_config &c = e->cfg;
     if (c.n_durations == 0) return e->fail(PK_ERR_INVALID, "pk_stream_open: streaming decodes a TDT joint; this is an RNN-T model");
+    // the cached attention reads position tables that cover the whole context (Tmax); a band engine keeps only -W..W
+    if (c.local_att_left || c.local_att_right) return e->fail(PK_ERR_INVALID, "pk_stream_open: not on a limited-context (local_att_*) engine");
     auto s = std::make_unique<StreamSet>();
     s->S = n_streams; s->L = att_context_left; s->R = att_context_right; s->max_chunk = max_chunk_samples;
     const int tot_max = 399 + max_chunk_samples;

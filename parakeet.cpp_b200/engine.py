@@ -33,7 +33,8 @@ class _PkConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "mel_bins", "sub_channels", "d_model", "n_layers", "n_heads", "ff", "conv_kernel", "vocab",
         "pred_hidden", "lstm_layers", "joint_hidden", "n_durations")] + [("durations", C.c_int32 * 8)] + \
-        [(n, C.c_int32) for n in ("has_ctc", "joint_prefix_tdt", "max_symbols", "max_batch", "max_samples", "math")]
+        [(n, C.c_int32) for n in ("has_ctc", "joint_prefix_tdt", "max_symbols", "max_batch", "max_samples", "math",
+                                  "local_att_left", "local_att_right")]
 
 
 class _PkSortformerConfig(C.Structure):
@@ -87,7 +88,7 @@ EXPORTS = ["pk_config_110m", "pk_config_tdt_600m", "pk_config_rnnt_600m", "pk_co
            "pk_transcribe_batch", "pk_stage_pcm", "pk_prefetch_pcm", "pk_run_staged", "pk_fetch_tokens", "pk_sync",
            "pk_token_buffer", "pk_stream", "pk_launch_count", "pk_profile_begin", "pk_profile_end",
            "pk_profile_names", "pk_flush_l2", "pk_selftest_gemm",
-           "pk_kernel_gemm", "pk_kernel_attention", "pk_kernel_layernorm", "pk_kernel_dwconv", "pk_kernel_ctc_argmax", "pk_kernel_tdt_decode", "pk_kernel_stream_attention", "pk_kernel_stream_dwconv",
+           "pk_kernel_gemm", "pk_kernel_attention", "pk_kernel_attention_local", "pk_kernel_layernorm", "pk_kernel_dwconv", "pk_kernel_ctc_argmax", "pk_kernel_tdt_decode", "pk_kernel_stream_attention", "pk_kernel_stream_dwconv",
            "pk_debug_tdt_phases", "pk_vocab_load", "pk_vocab_free", "pk_vocab_size",
            "pk_detokenize", "pk_group_words", "pk_tokenize", "pk_ctc_decode_boosted",
            "pk_resample_len", "pk_resample",
@@ -161,6 +162,7 @@ def load_library():
     L.pk_selftest_gemm.argtypes = [C.c_int] * 6 + [C.c_uint32, f32p, f32p]
     L.pk_kernel_gemm.argtypes = [C.c_int] * 10 + [C.c_float, C.c_int] + [f32p] * 7 + [i64p]
     L.pk_kernel_attention.argtypes = [C.c_int] * 4 + [i32p] + [C.c_int] * 4 + [f32p] * 7 + [i64p]
+    L.pk_kernel_attention_local.argtypes = [C.c_int] * 4 + [i32p] + [C.c_int] * 6 + [f32p] * 7 + [i64p]
     L.pk_kernel_layernorm.argtypes = [C.c_int] * 3 + [f32p] * 5 + [C.c_int] * 2 + [f32p] * 4 + [i64p]
     L.pk_kernel_dwconv.argtypes = [C.c_int] * 3 + [i32p] + [C.c_int] * 3 + [f32p] * 6 + [i64p]
     L.pk_kernel_ctc_argmax.argtypes = [C.c_int] * 4 + [f32p, i32p, f32p, f32p, i64p]
@@ -273,6 +275,10 @@ class ModelConfig:
     max_batch: int = 64
     max_samples: int = 160000
     math: int = int(Math.BF16X3)
+    # offline limited-context attention (left, right) for long utterances, NeMo's rel_pos_local_attn: frame i attends to
+    # frame j only when -right <= i - j <= left.  (0, 0) = full attention.  With a band, max_batch * max_samples may reach
+    # 3 h of audio (DESIGN.md section 16).  Separate from att_context_left / _right, which only pk_stream_open reads.
+    local_attention: tuple = (0, 0)
 
     def to_c(self) -> _PkConfig:
         c = _PkConfig()
@@ -286,6 +292,7 @@ class ModelConfig:
         c.joint_prefix_tdt = int(self.joint_prefix == "tdt_joint_.")
         c.max_symbols = self.max_symbols
         c.max_batch, c.max_samples, c.math = self.max_batch, self.max_samples, int(self.math)
+        c.local_att_left, c.local_att_right = (int(v) for v in self.local_attention)
         return c
 
     @property
